@@ -2,7 +2,7 @@
 """bench.py -- site-pattern conditional-likelihood updates per second (BASELINE.json's metric).
 
 Default workload (N=1): BASELINE.json configs[1] AS WRITTEN -- ONE analysis of primates.nex, 4-state
-GTR+G4, nruns=2 x nchains=4, all 8 chains on one B200: every generation one proposal per chain, the 8
+GTR+G4, nruns=2 x nchains=4, all 8 chains on one H100: every generation one proposal per chain, the 8
 chains evaluated in ONE chain-batched engine call = one fused kernel launch (P(t) rebuild for the dirty
 branches, pruning over the dirty nodes with the rescaler fused, root integration, lnL reduction), the
 accept step, and the Metropolis-coupling swap attempt (MC^3 shard coordinator, include/mb200_mc3.h).
@@ -550,7 +550,7 @@ def measured_peaks():
     pk = ROOT / "MEASURED_PEAKS.json"
     if pk.exists():
         return dict(json.loads(pk.read_text()), which="measured (MEASURED_PEAKS.json)")
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1650.0, "which": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "which": "H100 SXM data sheet (dense, 700 W)"}
 
 
 def kernel_roofline(torch, job, flush, peaks, device, max_launches=1024):
@@ -575,12 +575,12 @@ def kernel_roofline(torch, job, flush, peaks, device, max_launches=1024):
     avg_s = ms * 1e-3 / max(cnt, 1)
     ach = (tot_bytes / max(cnt, 1)) / avg_s / 1e9
     kind = "eval_nuc4_kernel<K=4,NT=256,FUSE> (4-state shuffle kernel)" if pr.S == 4 else \
-           f"eval_tcp_kernel<{pr.S}> (tcgen05, warp-specialised pipeline)" if pr.S in (20, 61) else "eval_gen_kernel"
+           f"eval_tcp_kernel<{pr.S}> (wgmma, warp-specialised pipeline)" if pr.S in (20, 61) else "eval_gen_kernel"
     if len(job.parts) > 1:
         kind += f" of partition {pi + 1} of {len(job.parts)} (the largest)"
     return {"bound": "hbm", "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": ach / peaks["hbm_gbs"],
-            "traffic": None, "traffic_note": "per-launch DRAM bytes: see the ncu captures under profiles/ (the working set of a "
-                                             "primates analysis, 2.7 MB, lives in L2; a constant here would not belong to this run)",
+            "traffic": None, "traffic_note": "per-launch DRAM bytes are not measured (the working set of a primates analysis, 2.7 MB, "
+                                             "lives in L2; a constant here would not belong to this run)",
             "kernel": kind, "avg_kernel_us": avg_s * 1e6, "launches_timed": cnt,
             "algorithmic_bytes_per_launch": tot_bytes / max(cnt, 1), "bytes_per_update": bytes_per_update(pr.S, pr.K),
             "peak_source": peaks["which"]}
@@ -630,7 +630,7 @@ def full_tree_workload(torch, lib, name, peaks, device, with_cpu=True):
                             "basis": "whole evaluation (P(t) kernels + pruning kernel), CUDA events on the instance's stream",
                             "pruning_kernel_ms": kms / max(kn, 1), "traffic": None,
                             "algorithmic_tflops": flops / (ms * 1e-3) / 1e12,
-                            "tensor_frac_3xtf32": (3.0 * flops / (ms * 1e-3) / 1e12) / (0.5 * peaks.get("bf16_tflops", 1650.0)) if S in (20, 61) else None}}
+                            "tensor_frac_3xtf32": (3.0 * flops / (ms * 1e-3) / 1e12) / (0.5 * peaks.get("bf16_tflops", 989.0)) if S in (20, 61) else None}}
     if with_cpu and REF_BIN.exists():
         try:
             rate, upd_c, wall, sec_c, desc = reference_sample(name, 1, 4321)
@@ -692,7 +692,7 @@ def bench_engine(args):
     peaks = measured_peaks()
     lib = abi.engine_library()
     if lib.fn("device_count")() < 1:
-        raise SystemExit("bench.py: no sm_100 device; the engine has no CPU fallback")
+        raise SystemExit("bench.py: no sm_90 device; the engine has no CPU fallback")
     hl = load_host_loop()
 
     name = args.workload
@@ -768,6 +768,8 @@ def bench_engine(args):
     b.record(); torch.cuda.synchronize()
     ms_reduce = a.elapsed_time(b)
     ms_value += ms_reduce
+    if args.dump_outputs:
+        dump_outputs(Path(args.dump_outputs), job, red, rank, world)
 
     # ---- e2e: host structs through the C-ABI ----
     barrier()
@@ -854,6 +856,18 @@ def bench_engine(args):
         dist.destroy_process_group()
 
 
+def dump_outputs(out: Path, job, run_sums, rank: int, world: int):
+    """What the timed leg hands its caller after its last step: every local chain's current lnL and lnPrior, the swap
+    statistics of the MC^3 coordinator, and the end-of-run reduce of the per-run lnL sums (rank 0)."""
+    out.mkdir(parents=True, exist_ok=True)
+    sfx = f"_rank{rank}" if world > 1 else ""
+    np.save(out / f"chain_lnl{sfx}.npy", np.asarray(job.cur_lnl, np.float64))
+    np.save(out / f"chain_lnprior{sfx}.npy", np.asarray(job.cur_lnpr, np.float64))
+    np.save(out / f"swap_info{sfx}.npy", job.mc.swap_info().astype(np.float64))
+    if rank == 0:
+        np.save(out / "run_lnl_sums.npy", np.asarray(run_sums, np.float64))
+
+
 class pack_bytes:
     """Size of the packed job a generation ships host->device (header + DevEval + rates/frequencies + branch
     list + node records).  Small jobs ride in the kernel parameter block, i.e. inside the launch."""
@@ -879,6 +893,8 @@ def main():
                     help="N=1 default workload only: large synthetic configs reported under other_workloads ('' = none)")
     ap.add_argument("--no-extras", action="store_true", help="skip many_analyses / other_workloads")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the value leg's outputs (per-chain lnL / lnPrior, per-run lnL sums) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         bench_reference(args)

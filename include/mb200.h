@@ -1,5 +1,5 @@
 /*
- * mb200.h -- C-ABI of the B200-native tree-likelihood engine for MrBayes.
+ * mb200.h -- C-ABI of the H100-native tree-likelihood engine for MrBayes.
  *
  * Plain C, plain pointers and sizes, no torch / CUDA types.  The library
  * (libmb200.so) owns every floating-point buffer of a data division on one
@@ -50,7 +50,7 @@
  *                                SURVEY.md section 8f-1)
  *
  * Every function returns MB200_SUCCESS (0) or a negative MB200_ERROR_* code;
- * there is no CPU fallback: without a usable sm_100 device
+ * there is no CPU fallback: without a usable sm_90 device
  * mb200_create_instance fails with MB200_ERROR_NO_DEVICE.
  */
 #ifndef MB200_H_
@@ -208,7 +208,7 @@ typedef struct mb200_evaluation
 int         mb200_abi_version (void);
 const char *mb200_version_string (void);
 const char *mb200_error_string (int code);
-int         mb200_device_count (void);     /* sm_100-class devices visible; 0 = none       */
+int         mb200_device_count (void);     /* sm_90-class devices visible; 0 = none        */
 
 /* ---- instance ---------------------------------------------------------------------- */
 int mb200_create_instance   (const mb200_instance_config *config, int *instance);
@@ -321,7 +321,7 @@ int mb200_get_stream       (int instance, void **stream);
 /* kernels launched by the instance since creation (bench.py's gpu_launches) */
 int mb200_get_launch_count (int instance, long long *launches);
 /* the same count per kernel family, so a caller (or a test) can tell WHICH path served it: the
- * 4-state shuffle kernel, the tcgen05 tensor-core kernel (20 / 61 states), the CUDA-core kernel for
+ * 4-state shuffle kernel, the wgmma tensor-core kernel (20 / 61 states), the CUDA-core kernel for
  * any other state count, the variable-state (Std) kernel, stand-alone P(t) builds, set-up kernels */
 #define MB200_KERNEL_NUC4     0
 #define MB200_KERNEL_TENSOR   1

@@ -1,4 +1,4 @@
-"""mrbayes_b200 -- B200-native tree-likelihood engine for MrBayes.
+"""mrbayes_b200 -- H100-native tree-likelihood engine for MrBayes.
 
 The product is the CUDA shared library ``mrbayes_b200/lib/libmb200.so`` (C-ABI:
 ``include/mb200.h``) plus the C seam ``mrbayes_b200/seam/`` that plugs it into MrBayes'

@@ -1,7 +1,7 @@
 """ctypes view of the C-ABI in include/mb200.h.
 
 Python is test and benchmark tooling here, not the product: the product is
-``mrbayes_b200/lib/libmb200.so`` (CUDA, sm_100a) called from MrBayes' C code through the
+``mrbayes_b200/lib/libmb200.so`` (CUDA, sm_90a) called from MrBayes' C code through the
 seam in ``mrbayes_b200/seam/``.  The same structs drive the CPU oracle
 (``oracle/liboracle.so``, ``orc_`` prefix) so that tests can feed identical inputs to both.
 

@@ -1,5 +1,5 @@
 // mb200_device.cuh -- device-side job format and buffer geometry shared by the kernels
-// and the host runtime of the B200 tree-likelihood engine.
+// and the host runtime of the H100 tree-likelihood engine.
 //
 // Data layout in HBM (per instance == one MrBayes data division on one GPU):
 //   tips      uint8  [tip][C]            (S <= 8)  state-set bitmask per pattern

@@ -1,8 +1,8 @@
-// mb200_engine.cu -- host runtime + C-ABI (include/mb200.h) of the B200 tree-likelihood
+// mb200_engine.cu -- host runtime + C-ABI (include/mb200.h) of the H100 tree-likelihood
 // engine.  Everything a data division needs lives in HBM for the life of the instance; a
 // likelihood evaluation moves a few hundred bytes of indices host->device and 12 bytes per
 // chain (lnL + status) device->host.  There is no CPU fallback in this file: without an
-// sm_100 device every entry point that needs the GPU fails.
+// sm_90 device every entry point that needs the GPU fails.
 #include "mb200.h"
 #include "mb200_device.cuh"
 #include "mb200_kernels.cuh"
@@ -57,7 +57,7 @@ struct Instance
     int          *dTipPartAmbig = nullptr;
     int           seq = 0;               // launch sequence number stamped into results
     float        *dSplit = nullptr;      // tensor-core path: pre-split (hi, lo) canonical images of every P(t)
-    int           tcS = 0;               // 20 or 61 when the tcgen05 kernel serves this instance, else 0
+    int           tcS = 0;               // 20 or 61 when the wgmma kernel serves this instance, else 0
     size_t        smemTc = 0;
     float        *dPartials = nullptr, *dMatrices = nullptr, *dScalers = nullptr, *dWeights = nullptr;
     double       *dEigen = nullptr;
@@ -85,7 +85,7 @@ struct Instance
     unsigned int *dTicket = nullptr;
     unsigned long long *dDbg = nullptr;
     bool          invMaskValid = false;
-    int           maxEval = 1, maxTiles = 1, numSMs = 148;
+    int           maxEval = 1, maxTiles = 1, numSMs = 132;
     size_t        eigenStride = 0;     // doubles per eigen slot (all parts)
     int           cijkParts = 1;       // eigensystems per slot (one per category for NY98-type models)
     size_t        smemGen = 0;         // dynamic smem of eval_gen_kernel
@@ -997,7 +997,7 @@ extern "C" {
 
 int mb200_abi_version (void) { return MB200_ABI_VERSION; }
 
-const char *mb200_version_string (void) { return "mb200 0.1 (sm_100a)"; }
+const char *mb200_version_string (void) { return "mb200 0.1 (sm_90a)"; }
 
 const char *mb200_error_string (int code)
 {
@@ -1007,7 +1007,7 @@ const char *mb200_error_string (int code)
         case MB200_ERROR_GENERAL:       return "general error";
         case MB200_ERROR_OUT_OF_MEMORY: return "out of device memory";
         case MB200_ERROR_OUT_OF_RANGE:  return "index or size out of range";
-        case MB200_ERROR_NO_DEVICE:     return "no sm_100 (B200) device available; the engine has no CPU fallback";
+        case MB200_ERROR_NO_DEVICE:     return "no sm_90 (H100) device available; the engine has no CPU fallback";
         case MB200_ERROR_UNSUPPORTED:   return "unsupported configuration";
         case MB200_ERROR_BAD_INSTANCE:  return "bad instance handle";
         case MB200_ERROR_CUDA:          return "CUDA runtime error";
@@ -1023,7 +1023,7 @@ int mb200_device_count (void)
     for (int d = 0; d < n; d++)
         {
         int major = 0;
-        if (cudaDeviceGetAttribute (&major, cudaDevAttrComputeCapabilityMajor, d) == cudaSuccess && major == 10)
+        if (cudaDeviceGetAttribute (&major, cudaDevAttrComputeCapabilityMajor, d) == cudaSuccess && major == 9)
             ok++;
         }
     return ok;
@@ -1046,14 +1046,14 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
     if (cfg->device < 0 || cfg->device >= n)
         return MB200_ERROR_NO_DEVICE;
     int major = 0, sms = 0;
-    if (cudaDeviceGetAttribute (&major, cudaDevAttrComputeCapabilityMajor, cfg->device) != cudaSuccess || major != 10)
-        return MB200_ERROR_NO_DEVICE;        // kernels exist for sm_100a only
+    if (cudaDeviceGetAttribute (&major, cudaDevAttrComputeCapabilityMajor, cfg->device) != cudaSuccess || major != 9)
+        return MB200_ERROR_NO_DEVICE;        // kernels exist for sm_90a only
     CK (cudaSetDevice (cfg->device));
     cudaDeviceGetAttribute (&sms, cudaDevAttrMultiProcessorCount, cfg->device);
 
     Instance *I = new Instance ();
     I->cfg = *cfg;
-    I->numSMs = sms > 0 ? sms : 148;
+    I->numSMs = sms > 0 ? sms : 132;
     I->maxEval = cfg->max_evaluations > 0 ? cfg->max_evaluations : 1;
     const int S = cfg->state_count, K = cfg->category_count, C = cfg->pattern_count;
     const int Sp = (S + 3) & ~3;
@@ -1079,8 +1079,8 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
         { delete I; return MB200_ERROR_OUT_OF_RANGE; }      // 4-state records carry 32-bit element offsets (64 GB of partials)
     if (!getenv ("MB200_DISABLE_TC") && !I->std)
         {
-        if (S == 61 && K <= 3) I->tcS = 61;      // 61-state codon (K > 1: omega categories, NY98 / M3), tcgen05 path
-        if (S == 20 && K <= 4) I->tcS = 20;      // 20-state amino acids, tcgen05 path
+        if (S == 61 && K <= 3) I->tcS = 61;      // 61-state codon (K > 1: omega categories, NY98 / M3), wgmma path
+        if (S == 20 && K <= 4) I->tcS = 20;      // 20-state amino acids, wgmma path
         }
     int stdLanes = 1;
     while (stdLanes < K) stdLanes <<= 1;

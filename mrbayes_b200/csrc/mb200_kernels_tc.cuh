@@ -1,20 +1,20 @@
-// mb200_kernels_tc.cuh -- what the tensor-core (tcgen05 / TMEM) pruning path shares: operand geometry, the pre-split
+// mb200_kernels_tc.cuh -- what the tensor-core (wgmma) pruning path shares: operand geometry, the pre-split
 // P(t) operand images, the node-parallel work queue.  The kernel itself is eval_tcp_kernel (mb200_kernels_tcp.cuh).
 // It serves the state counts where a node update really is a dense contraction: 20-state amino-acid and 61-state codon
 // models (CondLikeDown/Root_Gen*, _NY98*, CondLikeScaler_Gen*, Likelihood_Gen*; reference src/likelihood.c:204, 1575,
 // 2152, 4010, 4939, 5764).
 //
 // Per node, per rate category, per child:   D[128 patterns][S] = CL_child[128][S] * P^T[S][S]
-// is a 128 x NP x KP tcgen05.mma chain (kind::tf32, FP32 accumulate in TMEM), NP/KP = S padded to
-// the MMA granularity (61 -> 64/64, 20 -> 32/24).  FP32 accuracy is recovered with the 3xTF32 split
+// is a chain of wgmma.mma_async (two 64-row warpgroup halves, kind tf32, FP32 accumulators in registers), NP/KP = S
+// padded to the MMA granularity (61 -> 64/64, 20 -> 32/24).  FP32 accuracy is recovered with the 3xTF32 split
 //     x = hi + lo,  hi = rna_tf32(x),  lo = rna_tf32(x - hi):   A*B ~= Ahi*Bhi + (Ahi*Blo + Alo*Bhi)
-// (plain TF32 would cost ~2e-4 per product; the split leaves ~7e-7, see tests/probes/umma_probe.cu).
-// The large term and the two small correction terms go to SEPARATE TMEM accumulators so that the
+// (plain TF32 would cost ~2e-4 per product; the split leaves ~7e-7).
+// The large term and the two small correction terms go to SEPARATE accumulators so that the
 // tensor core's truncating accumulation bias is paid on KP/8 steps only, and are added in FP32 (RN)
 // in the epilogue.
 #pragma once
 #include "mb200_device.cuh"
-#include "umma_common.cuh"
+#include "gmma_common.cuh"
 
 template <int S> struct TcGeom;
 template <> struct TcGeom<61> { static constexpr int NP = 64, KP = 64, SP = 64; };
@@ -30,9 +30,9 @@ template <int S>
 __device__ __forceinline__ void tc_write_split_entry (float *img, int i, int j, float p)
 {
     constexpr int NP = TcGeom<S>::NP;
-    const float hi = umma::to_tf32 (p), lo = umma::to_tf32 (p - hi);
-    img[umma::canon_off (i, j, 2 * NP) / 4] = hi;
-    img[umma::canon_off (NP + i, j, 2 * NP) / 4] = lo;
+    const float hi = gmma::to_tf32 (p), lo = gmma::to_tf32 (p - hi);
+    img[gmma::canon_off (i, j, 2 * NP) / 4] = hi;
+    img[gmma::canon_off (NP + i, j, 2 * NP) / 4] = lo;
 }
 
 // split images of matrices already present in the matrix buffer (set_transition_matrix, or a

@@ -1,10 +1,10 @@
-// mb200_kernels_tcp.cuh -- warp-specialised, pipelined tcgen05 pruning kernel (eval_tcp_kernel) for the 20-state
+// mb200_kernels_tcp.cuh -- warp-specialised, pipelined wgmma pruning kernel (eval_tcp_kernel) for the 20-state
 // amino-acid and 61-state codon paths (CondLikeDown/Root_Gen*, _NY98*, CondLikeScaler_Gen*, Likelihood_Gen*/_NY98*;
 // reference src/likelihood.c:204, 1575, 2152, 4010, 4939, 5413, 5764, 6975).
 //
 // Work = (node, 128-pattern tile) items of the device-side queue of mb200_kernels_tc.cuh (level order, acquire /
 // release flags between the CTAs of a persistent grid).  Inside the CTA the phases of an item do not run back to
-// back: one CTA per SM, 20 warps with fixed roles, mbarrier rings between them.
+// back: one CTA per SM, 18 warps with fixed roles, mbarrier rings between them.
 //
 //   scheduler (1 warp)    draws tickets, decodes (slot, evaluation, tile), waits for the item's producers (flag
 //                         acquire), publishes the item in a 4-deep shared-memory ring
@@ -13,16 +13,15 @@
 //                         (512-byte coalesced LDG.128) -> hi/lo TF32 split -> canonical K-major core-matrix images in
 //                         an operand-ring stage; the branch's pre-split P(t) image [hi | lo] arrives in the same stage by
 //                         one bulk async copy (TMA engine, complete_tx on the stage's full barrier)
-//   MMA       (1 warp)    per unit: [main | corr] = A_hi x [B_hi | B_lo]^T  (ONE tcgen05.mma chain, N = 2 NP) and
-//                         corr += A_lo x B_hi^T (N = NP) into one slot of a TMEM accumulator ring; tcgen05.commit
-//                         frees the operand stage and hands the accumulators to the epilogue
-//   epilogue  (2 x 4)     two halves share an item: thread = pattern row = TMEM lane, the 16-column strips of a row
-//                         alternate between the halves: tcgen05.ld, main + corr, product over the children, row maximum;
-//                         unscaled rows staged in shared memory, then coalesced 16-byte stores of row * (1 / max) -- the
-//                         two roundings of the reference's rescaler; node scaler; the evaluation's closing item (site
-//                         scalers, root integration, lnL tile sums) runs here too
+//   consumers (2 x 4)     two warpgroups, one per 64-row half of the tile.  Per unit: [main | corr] = A_hi x [B_hi | B_lo]^T
+//                         (ONE wgmma chain, N = 2 NP) and corr += A_lo x B_hi^T (N = NP), accumulators in registers; once
+//                         the MMAs have completed the operand stage goes back to the loaders.  Then main + corr, product
+//                         over the children (kept in the shared-memory staging area), row maximum; after the last child
+//                         coalesced 16-byte stores of row * (1 / max) -- the two roundings of the reference's rescaler;
+//                         node scaler; the evaluation's closing item (site scalers, root integration, lnL tile sums)
+//                         runs here too
 //   publisher (1 warp)    release-stores the node-done flags (the memory barrier of a release does not stall a warp that
-//                         has accumulators waiting)
+//                         has the next item's operands waiting)
 //
 // 3xTF32 as before (x = hi + lo, lo x lo dropped); the large term and the two correction terms land in separate
 // accumulators and are added in FP32 in the epilogue.
@@ -30,12 +29,12 @@
 #include "mb200_kernels_tc.cuh"
 
 template <int S> struct TcpGeom;
-// NA: TMEM ring, NA units x 2 NP columns = 512.  LG: loader groups (8 / LG warps each) -- units go round-robin to the
-// groups, so LG units' loads are in flight per SM; a 20-state unit is small (10 KB), hence more, smaller groups
-template <> struct TcpGeom<61> { static constexpr int NA = 4, LG = 2; };
-template <> struct TcpGeom<20> { static constexpr int NA = 8, LG = 4; };
+// LG: loader groups (8 / LG warps each) -- units go round-robin to the groups, so LG units' loads are in flight per SM;
+// a 20-state unit is small (30 KB), hence more, smaller groups
+template <> struct TcpGeom<61> { static constexpr int LG = 2; };
+template <> struct TcpGeom<20> { static constexpr int LG = 4; };
 
-constexpr int TCP_THREADS   = 608;     // 2 x 4 epilogue warps, 8 loader warps, MMA issuer, scheduler, publisher
+constexpr int TCP_THREADS   = 576;     // 2 x 4 consumer warps, 8 loader warps, scheduler, publisher
 constexpr int TCP_NPUB      = 4;       // flag-publication ring (epilogue -> publisher warp)
 constexpr int TCP_NS_MAX    = 8;       // operand-ring stages (as many as fit beside the staging area)
 constexpr int TCP_NI        = 4;       // item ring
@@ -57,8 +56,9 @@ template <int S> __host__ __device__ constexpr size_t tcp_staging_bytes (int K)
 {
     return (size_t) K * ((S + 3) / 4) * 129 * sizeof(float4);   // one item's result rows, [k][16-byte chunk][row + pad]
 }
-// "this row's tip is fully ambiguous" bytes, one 128-byte record per unit in flight (loader -> epilogue)
-template <int S> __host__ __device__ constexpr size_t tcp_tipring_bytes (int NS) { return (size_t)(TcpGeom<S>::NA + NS) * 128; }
+// "this row's tip is fully ambiguous" bytes, one 128-byte record per operand-ring stage (loader -> consumers; read
+// before the stage is handed back)
+template <int S> __host__ __device__ constexpr size_t tcp_tipring_bytes (int NS) { return (size_t) NS * 128; }
 // stages that fit in `limit` bytes of dynamic shared memory: a multiple of the loader groups (every stage is then
 // always filled by the same group, which sees each of its phases -- the parity wait cannot alias), or 1: one group
 // loads everything
@@ -80,7 +80,7 @@ template <int S> inline int tcp_stages (int K, size_t limit)
 // with an error instead of sitting on the GPU until somebody's watchdog fires)
 __device__ __forceinline__ void tcp_wait (uint64_t *bar, uint32_t parity)
 {
-    const uint32_t a = umma::smem_u32 (bar);
+    const uint32_t a = gmma::smem_u32 (bar);
     uint32_t done = 0;
     unsigned long long t0 = 0;
     for (unsigned it = 0; ; it++)
@@ -124,10 +124,9 @@ __global__ void __launch_bounds__(TCP_THREADS, 1)
 eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ evals, const double *__restrict__ dvals,
                  const DevOp *__restrict__ ops, const float *__restrict__ split, DevResult *out, int seq)
 {
-    using namespace umma;
-    constexpr int NP = TcGeom<S>::NP, KP = TcGeom<S>::KP, NA = TcpGeom<S>::NA;
+    using namespace gmma;
+    constexpr int NP = TcGeom<S>::NP, KP = TcGeom<S>::KP;
     constexpr int TM = 128;
-    constexpr int UC = 2 * NP;                                  // TMEM columns of one unit: [main | corr]
     constexpr uint32_t LBO_A = (TM / 8) * 128, LBO_B = (2 * NP / 8) * 128, SBO = 128;
     constexpr int A_FLOATS = TM * KP;
     constexpr int B_FLOATS = 2 * NP * KP;
@@ -136,41 +135,34 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
     constexpr size_t STAGE = tcp_stage_bytes<S> ();
 
     extern __shared__ __align__(128) unsigned char tcp_smem[];
-    __shared__ uint64_t barFull[TCP_NS_MAX], barEmpty[TCP_NS_MAX], barAccFull[NA], barAccEmpty[NA], barInfoFull[TCP_NI], barInfoEmpty[TCP_NI];
+    __shared__ uint64_t barFull[TCP_NS_MAX], barEmpty[TCP_NS_MAX], barInfoFull[TCP_NI], barInfoEmpty[TCP_NI];
     __shared__ TcpItem sInfo[TCP_NI];
-    __shared__ uint32_t tmemBase;
     __shared__ uint64_t barPubFull[TCP_NPUB], barPubEmpty[TCP_NPUB];
     __shared__ int   *sPub[TCP_NPUB];  // flags to release, in order (nullptr: stop)
-    __shared__ float  sMax[2][TM];     // row maxima found by the two epilogue halves
+    __shared__ float  sMax[TM];        // row maxima (each row belongs to one consumer warpgroup)
     __shared__ double qSum[2][4];
     __shared__ int    qAb[2][4];
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int Sp = ctx.Sp, K = ctx.K, C = ctx.C;
-    float4 *sStage = reinterpret_cast<float4 *>(tcp_smem + (size_t) NS * STAGE);     // [group][buffer][chunk][TM+1]
-    const int TIPRING = NA + NS;
+    float4 *sStage = reinterpret_cast<float4 *>(tcp_smem + (size_t) NS * STAGE);     // [k][chunk][TM+1]
+    const int TIPRING = NS;
     unsigned char *sTipFull = tcp_smem + (size_t) NS * STAGE + tcp_staging_bytes<S> (K);   // [unit % TIPRING][row]
 
-    if (warp == 0)
-        tmem_alloc<512> (&tmemBase);
     if (tid == 32)
         {
-        for (int s = 0; s < NS; s++) { mbar_init (&barFull[s], 8 / TcpGeom<S>::LG + 1); mbar_init (&barEmpty[s], 1); }
-        for (int a = 0; a < NA; a++) { mbar_init (&barAccFull[a], 2); mbar_init (&barAccEmpty[a], 8); }
-        for (int i = 0; i < TCP_NI; i++) { mbar_init (&barInfoFull[i], 1); mbar_init (&barInfoEmpty[i], 17); }
+        for (int s = 0; s < NS; s++) { mbar_init (&barFull[s], 8 / TcpGeom<S>::LG + 1); mbar_init (&barEmpty[s], 8); }
+        for (int i = 0; i < TCP_NI; i++) { mbar_init (&barInfoFull[i], 1); mbar_init (&barInfoEmpty[i], 16); }
         for (int i = 0; i < TCP_NPUB; i++) { mbar_init (&barPubFull[i], 1); mbar_init (&barPubEmpty[i], 1); }
         mbar_fence_init ();
         }
-    fence_before_sync ();
     __syncthreads ();
-    fence_after_sync ();
-    const uint32_t tBase = tmemBase;
     const size_t bufStride = (size_t)K * C * Sp;
     const int rows = TM, numTiles = ctx.numTiles;
     const int perSlot = Q.nEval * numTiles;
     const int total = (Q.maxOps + 1) * perSlot;
 
-    if (warp == 17)
+    if (warp == 16)
         {
         // =================================================================== scheduler
         int slot = 0; uint32_t ph = 0;
@@ -357,7 +349,7 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                                 }
                             }
                         }
-                    fence_async_smem ();                        // generic-proxy stores -> async proxy (tcgen05.mma)
+                    fence_async_smem ();                        // generic-proxy stores -> async proxy (wgmma)
                     __syncwarp ();
                     if (lane == 0) mbar_arrive (&barFull[s]);
 #ifndef TCP_TRACE_EPI
@@ -368,62 +360,7 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
             nItem++;
             }
         }
-    else if (warp == 16)
-        {
-        // =================================================================== MMA issuer
-        constexpr uint32_t idescWide = make_idesc_tf32 (TM, 2 * NP), idescNarrow = make_idesc_tf32 (TM, NP);
-        constexpr uint64_t A_LO = (A_FLOATS * 4) >> 4, A_KS = (2 * LBO_A) >> 4, B_KS = (2 * LBO_B) >> 4, ST = STAGE >> 4;
-        const uint64_t dA0 = make_desc (smem_u32 (tcp_smem), LBO_A, SBO);
-        const uint64_t dB0 = make_desc (smem_u32 (tcp_smem + 2 * A_FLOATS * 4), LBO_B, SBO);
-        int islot = 0; uint32_t iph = 0;
-        unsigned u = 0;
-        unsigned nItem = 0;
-        for (;;)
-            {
-            tcp_wait (&barInfoFull[islot], iph);
-            const int kind = sInfo[islot].kind, nChild = sInfo[islot].nChild;
-            const int c1 = sInfo[islot].child[0], c2 = sInfo[islot].child[1], c3 = sInfo[islot].child[2];
-            __syncwarp ();
-            if (lane == 0) mbar_arrive (&barInfoEmpty[islot]);
-            if (++islot == TCP_NI) { islot = 0; iph ^= 1; }
-            if (kind == TCP_ITEM_STOP) break;
-            if (kind == TCP_ITEM_CLOSE) { nItem++; continue; }
-            for (int k = 0; k < K; k++)
-                for (int ch = 0; ch < nChild; ch++, u++)
-                    {
-                    const int s = (int)(u % (unsigned) NS), a = (int)(u % (unsigned) NA);
-                    const uint32_t ph = (u / (unsigned) NS) & 1u, aph = (u / (unsigned) NA) & 1u;
-                    const bool isTip = ((ch == 0) ? c1 : (ch == 1) ? c2 : c3) < ctx.tipCount;
-                    tcp_wait (&barFull[s], ph);                 // operand images (generic stores + bulk copy) have landed
-                    if (lane == 0 && k == 0 && ch == 0) TCP_T (nItem, 8);
-                    tcp_wait (&barAccEmpty[a], aph ^ 1);        // the epilogue has drained this accumulator slot
-                    if (lane == 0 && k == 0 && ch == 0) TCP_T (nItem, 9);
-                    fence_after_sync ();
-                    if (lane == 0)
-                        {
-                        const uint64_t aHi = dA0 + (uint64_t) s * ST, aLo = aHi + A_LO, bb = dB0 + (uint64_t) s * ST;
-                        const uint32_t tAcc = tBase + (uint32_t)(a * UC);
-                        #pragma unroll
-                        for (int ks = 0; ks < KP / 8; ks++)
-                            mma_tf32 (tAcc, aHi + ks * A_KS, bb + ks * B_KS, idescWide, ks > 0);
-                        if (!isTip)
-                            {
-                            #pragma unroll
-                            for (int ks = 0; ks < KP / 8; ks++)
-                                mma_tf32 (tAcc + NP, aLo + ks * A_KS, bb + ks * B_KS, idescNarrow, true);
-                            }
-                        mma_commit (&barEmpty[s]);              // operand stage free once these MMAs have read it
-                        mma_commit (&barAccFull[a]);            // accumulators complete ...
-                        mbar_arrive (&barAccFull[a]);           // ... and what this thread has seen (the loaders' shared-memory
-                                                                // writes, acquired with the stage) is released to the epilogue
-                        if (k == K - 1 && ch == nChild - 1) TCP_T (nItem, 10);
-                        }
-                    __syncwarp ();
-                    }
-            nItem++;
-            }
-        }
-    else if (warp == 18)
+    else if (warp == 17)
         {
         // =================================================================== publisher: release-stores the node-done flags,
         // so that no epilogue warp sits in a memory barrier
@@ -446,18 +383,17 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
         }
     else
         {
-        // =================================================================== epilogue: two halves of four warps share every
-        // item -- thread = pattern row = TMEM lane in both, the 16-column strips of a row alternate between them; the
-        // products are staged UNSCALED in shared memory ([k][chunk][row]: conflict-free for thread = row), the halves
-        // exchange their row maxima, and all 256 threads copy the rows out with coalesced 16-byte stores of
-        // row * (1 / max) -- the two roundings of CondLikeScaler_Gen (src/likelihood.c:4939-4990).
+        // =================================================================== consumers: warpgroup g = rows [64 g, 64 g + 64)
+        // of every item.  The products are staged UNSCALED in shared memory ([k][chunk][row]), the row maxima meet in
+        // sMax, and all 256 threads copy the rows out with coalesced 16-byte stores of row * (1 / max) -- the two
+        // roundings of CondLikeScaler_Gen (src/likelihood.c:4939-4990).
+        constexpr uint64_t A_LO = (A_FLOATS * 4) >> 4, A_KS = (2 * LBO_A) >> 4, B_KS = (2 * LBO_B) >> 4;
         const int grp = warp >> 2, gtid = tid & (TM - 1), row = gtid;
-        const uint32_t laneSel = (uint32_t)((warp & 3) * 32) << 16;
+        const int fRow = grp * 64 + (warp & 3) * 16 + (lane >> 2), fCol = 2 * (lane & 3);   // accumulator fragment
         int islot = 0; uint32_t iph = 0;
         int pslot = 0; uint32_t pph = 0;
         unsigned u = 0;
         unsigned nItem = 0;
-        unsigned accPar = 0;                                    // parity of the next phase of barAccFull[slot], one bit per slot
         for (;; nItem++)
             {
             tcp_wait (&barInfoFull[islot], iph);
@@ -487,95 +423,83 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
 
             if (it.kind == TCP_ITEM_NODE)
                 {
-                float mx = 0.0f;
-                // preLike shortcut of the scalar kernels (src/likelihood.c:257-258): a fully ambiguous tip contributes exactly 1
-                const unsigned tipKids = it.shortcut ? ((ch0 < ctx.tipCount ? 1u : 0u) | (ch1 < ctx.tipCount ? 2u : 0u) |
-                                                        ((it.nChild > 2 && ch2 < ctx.tipCount) ? 4u : 0u)) : 0u;
+                float mx[2] = { 0.0f, 0.0f };                   // fragment rows fRow, fRow + 8
                 for (int k = 0; k < K; k++)
-                    {
-                    // the accumulators of all children of (item, k) sit in consecutive slots of the TMEM ring: wait for
-                    // the last one (commits complete in issue order), then combine 16 columns at a time
-                    for (int ch = 0; ch < it.nChild; ch++)
+                    for (int ch = 0; ch < it.nChild; ch++, u++)
                         {
-                        const int a = (int)((u + ch) % (unsigned) NA);
-                        tcp_wait (&barAccFull[a], (accPar >> a) & 1u);
-                        accPar ^= 1u << a;
-                        }
-                    fence_after_sync ();
-                    if (gtid == 0 && k == K - 1) TCP_T (nItem, 12);
-                    unsigned tipFull = 0;
-                    if (tipKids)
-                        {
-                        if (tipKids & 1u) tipFull |= sTipFull[(u % (unsigned) TIPRING) * 128 + row] ? 1u : 0u;
-                        if (tipKids & 2u) tipFull |= sTipFull[((u + 1) % (unsigned) TIPRING) * 128 + row] ? 2u : 0u;
-                        if (tipKids & 4u) tipFull |= sTipFull[((u + 2) % (unsigned) TIPRING) * 128 + row] ? 4u : 0u;
-                        }
-                    const uint32_t tA0 = tBase + (uint32_t)((int)(u % (unsigned) NA) * UC) + laneSel;
-                    const uint32_t tA1 = tBase + (uint32_t)((int)((u + 1) % (unsigned) NA) * UC) + laneSel;
-                    const uint32_t tA2 = tBase + (uint32_t)((int)((u + 2) % (unsigned) NA) * UC) + laneSel;
-                    #pragma unroll
-                    for (int cb = 0; cb < NP; cb += 16)
-                        {
-                        if (cb >= S) break;
-                        if ((((cb >> 4) + k) & 1) != grp) continue;     // the other half's strip
-                        float prod[16];
-                        {
-                        // the first two children's strips are read together: four TMEM loads in flight, one wait
-                        uint32_t vm0[16], vc0[16], vm1[16], vc1[16];
-                        tmem_ld16_nowait (tA0 + cb, vm0);
-                        tmem_ld16_nowait (tA0 + NP + cb, vc0);
-                        tmem_ld16_nowait (tA1 + cb, vm1);
-                        tmem_ld16_nowait (tA1 + NP + cb, vc1);
-                        tmem_ld_wait ();
+                        const int s = (int)(u % (unsigned) NS);
+                        const int child = (ch == 0) ? ch0 : (ch == 1) ? ch1 : ch2;
+                        const bool isTip = child < ctx.tipCount;
+                        tcp_wait (&barFull[s], (u / (unsigned) NS) & 1u);   // operand images (generic stores + bulk copy) have landed
+                        if (tid == 0 && k == 0 && ch == 0) TCP_T (nItem, 8);
+                        const uint32_t st = smem_u32 (tcp_smem + (size_t) s * STAGE);
+                        const uint64_t aHi = make_desc (st + grp * (64 / 8) * 128, LBO_A, SBO), aLo = aHi + A_LO;
+                        const uint64_t bb  = make_desc (st + 2 * A_FLOATS * 4, LBO_B, SBO);
+                        float acc[NP];                          // [main | corr] columns of this thread's fragment
                         #pragma unroll
-                        for (int i = 0; i < 16; i++)
+                        for (int i = 0; i < NP; i++) { acc[i] = 0.0f; fence_regs (acc[i]); }
+                        mma_fence ();
+                        #pragma unroll
+                        for (int ks = 0; ks < KP / 8; ks++)
+                            mma_tf32<2 * NP> (acc, aHi + ks * A_KS, bb + ks * B_KS, ks > 0);
+                        if (!isTip)
                             {
-                            float v0 = __uint_as_float (vm0[i]) + __uint_as_float (vc0[i]);
-                            float v1 = __uint_as_float (vm1[i]) + __uint_as_float (vc1[i]);
-                            if (tipFull & 1u) v0 = 1.0f;
-                            if (tipFull & 2u) v1 = 1.0f;
-                            prod[i] = v0 * v1;
-                            }
-                        }
-                        if (it.nChild > 2)
-                            {
-                            uint32_t vm[16], vc[16];
-                            tmem_ld16_nowait (tA2 + cb, vm);
-                            tmem_ld16_nowait (tA2 + NP + cb, vc);
-                            tmem_ld_wait ();
                             #pragma unroll
-                            for (int i = 0; i < 16; i++)
+                            for (int ks = 0; ks < KP / 8; ks++)
+                                mma_tf32<NP> (acc + NP / 2, aLo + ks * A_KS, bb + ks * B_KS, true);
+                            }
+                        mma_commit ();
+                        mma_wait_all ();
+                        #pragma unroll
+                        for (int i = 0; i < NP; i++) fence_regs (acc[i]);
+                        // preLike shortcut of the scalar kernels (src/likelihood.c:257-258): a fully ambiguous tip contributes exactly 1
+                        bool tipFull[2] = { false, false };
+                        if (it.shortcut && isTip)
+                            {
+                            tipFull[0] = sTipFull[(u % (unsigned) TIPRING) * 128 + fRow] != 0;
+                            tipFull[1] = sTipFull[(u % (unsigned) TIPRING) * 128 + fRow + 8] != 0;
+                            }
+                        __syncwarp ();
+                        if (lane == 0) mbar_arrive (&barEmpty[s]);     // operands read: the stage goes back to the loaders
+                        if (tid == 0 && k == K - 1 && ch == it.nChild - 1) TCP_T (nItem, 12);
+                        const bool last = ch == it.nChild - 1;
+                        #pragma unroll
+                        for (int j = 0; j < NP / 8; j++)
+                            {
+                            const int col = 8 * j + fCol;
+                            if (col >= 4 * NQ) continue;        // padding columns beyond the staged chunks
+                            #pragma unroll
+                            for (int h = 0; h < 2; h++)
                                 {
-                                float v = __uint_as_float (vm[i]) + __uint_as_float (vc[i]);
-                                if (tipFull & 4u) v = 1.0f;
-                                prod[i] *= v;
+                                float v0 = acc[4 * j + 2 * h] + acc[NP / 2 + 4 * j + 2 * h];
+                                float v1 = acc[4 * j + 2 * h + 1] + acc[NP / 2 + 4 * j + 2 * h + 1];
+                                if (tipFull[h]) { v0 = 1.0f; v1 = 1.0f; }
+                                float2 *p = reinterpret_cast<float2 *>(reinterpret_cast<float *>(sStage) +
+                                                                       (((size_t)k * NQ + col / 4) * (TM + 1) + fRow + 8 * h) * 4 + (col & 3));
+                                if (ch > 0)
+                                    {
+                                    const float2 o = *p;        // product of the earlier children (this thread wrote it)
+                                    v0 = o.x * v0; v1 = o.y * v1;
+                                    }
+                                if (last)
+                                    {
+                                    if (col >= S) v0 = 0.0f;
+                                    if (col + 1 >= S) v1 = 0.0f;
+                                    mx[h] = fmaxf (mx[h], fmaxf (v0, v1));
+                                    }
+                                *p = make_float2 (v0, v1);
                                 }
                             }
-                        #pragma unroll
-                        for (int i = 0; i < 16; i++)
-                            if (cb + i < S) mx = fmaxf (mx, prod[i]);
-                        #pragma unroll
-                        for (int j = 0; j < 4; j++)
-                            if (cb + j*4 < S)
-                                {
-                                float4 v;
-                                v.x = prod[j*4];
-                                v.y = (cb + j*4 + 1 < S) ? prod[j*4 + 1] : 0.f;
-                                v.z = (cb + j*4 + 2 < S) ? prod[j*4 + 2] : 0.f;
-                                v.w = (cb + j*4 + 3 < S) ? prod[j*4 + 3] : 0.f;
-                                sStage[((size_t)k * NQ + cb / 4 + j) * (TM + 1) + row] = v;
-                                }
                         }
-                    fence_before_sync ();                       // TMEM reads ordered before the slots' next MMAs
-                    __syncwarp ();
-                    if (lane == 0)
-                        for (int ch = 0; ch < it.nChild; ch++)
-                            mbar_arrive (&barAccEmpty[(int)((u + ch) % (unsigned) NA)]);
-                    u += (unsigned) it.nChild;
+                #pragma unroll
+                for (int h = 0; h < 2; h++)
+                    {
+                    mx[h] = fmaxf (mx[h], __shfl_xor_sync (0xffffffffu, mx[h], 1));
+                    mx[h] = fmaxf (mx[h], __shfl_xor_sync (0xffffffffu, mx[h], 2));
                     }
+                if ((lane & 3) == 0) { sMax[fRow] = mx[0]; sMax[fRow + 8] = mx[1]; }
                 if (tid == 0) TCP_T (nItem, 13);
-                // the halves meet: row maxima, then the copy-out
-                sMax[grp][row] = mx;
+                // the warpgroups meet: row maxima, then the copy-out
                 tcp_bar_epilogue ();
                 const bool doScale = it.sw >= 0;
                 {
@@ -589,7 +513,7 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                     {
                     const int idx = n * 256 + tid;
                     const int r = (idx < nq * TM) ? idx / nq : 0;
-                    fr[n] = doScale ? __frcp_rn (fmaxf (sMax[0][r], sMax[1][r])) : 1.0f;      // = 1.0f / max, IEEE
+                    fr[n] = doScale ? __frcp_rn (sMax[r]) : 1.0f;      // = 1.0f / max, IEEE
                     }
                 for (int k = 0; k < K; k++)
                     {
@@ -615,7 +539,7 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                     }
                 }
                 if (doScale && grp == 0 && active)              // node scaler (CondLikeScaler_Gen_SSE: log in double, cast to float, src/likelihood.c:5055)
-                    ctx.scalers[(size_t)it.sw * C + c] = log_of_max (fmaxf (sMax[0][row], sMax[1][row]));
+                    ctx.scalers[(size_t)it.sw * C + c] = log_of_max (sMax[row]);
                 // publish: the barrier orders every epilogue thread's stores before thread 0's hand-over; the publisher warp
                 // acquires it and release-stores the flag (cumulative at GPU scope), so no epilogue warp sits in a memory
                 // barrier while the next item's accumulators are waiting
@@ -722,8 +646,4 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
             }
         }
 
-    fence_before_sync ();
-    __syncthreads ();
-    if (warp == 0)
-        tmem_dealloc<512> (tmemBase);
 }

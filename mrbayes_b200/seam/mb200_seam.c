@@ -1,5 +1,5 @@
 /*
- * mb200_seam.c -- host-side seam between MrBayes' C code and the B200 engine.
+ * mb200_seam.c -- host-side seam between MrBayes' C code and the H100 engine.
  *
  * This translation unit is compiled TOGETHER WITH the reference's headers
  * (-I<mrbayes>/src) and linked into the reference's `mb` binary.  It
@@ -744,7 +744,7 @@ int InitBeagleInstance (ModelInfo *m, int division)
     rc = seamBackend.create_instance (&cfg, &inst);
     if (rc != MB200_SUCCESS)
         {
-        MrBayesPrint ("%s   B200 engine: cannot create instance for division %d (%s)\n", spacer, division+1, mb200_error_string (rc));
+        MrBayesPrint ("%s   H100 engine: cannot create instance for division %d (%s)\n", spacer, division+1, mb200_error_string (rc));
         inst = -1;
         goto fail;
         }
@@ -807,12 +807,12 @@ int InitBeagleInstance (ModelInfo *m, int division)
     sd->hostPFailed = NO;
     if (seamBatchWanted == YES && numLocalChains > 1 && SeamBuildScratchSets (m, sd) == ERROR)
         {
-        MrBayesPrint ("%s   B200 engine: cannot build the per-chain scratch sets of division %d\n", spacer, division+1);
+        MrBayesPrint ("%s   H100 engine: cannot build the per-chain scratch sets of division %d\n", spacer, division+1);
         SeamDropDivision (division);
         return (ERROR);
         }
 
-    MrBayesPrint ("%s   Using B200 engine (%s) for division %d on device %d: %d patterns x %d categories x %d states\n",
+    MrBayesPrint ("%s   Using H100 engine (%s) for division %d on device %d: %d patterns x %d categories x %d states\n",
                   spacer, mb200_version_string (), division+1, cfg.device, m->numChars, SeamCategories (m), m->numModelStates);
     return (NO_ERROR);
 
@@ -1278,7 +1278,7 @@ static int SeamApplyResult (int division, int chain, int rc, double value, int s
         }
     if (rc != MB200_SUCCESS)
         {
-        MrBayesPrint ("%s   B200 engine: evaluation failed for division %d (%s)\n", spacer, division+1, mb200_error_string (rc));
+        MrBayesPrint ("%s   H100 engine: evaluation failed for division %d (%s)\n", spacer, division+1, mb200_error_string (rc));
         (*lnL) = MRBFLT_NEG_MAX;
         abortMove = YES;
         return (ERROR);
@@ -1828,7 +1828,7 @@ void LaunchBEAGLELogLikeMultiPartition (int *divisions, int divisionCount, int c
             memset (seamCijkSeen[d], 0, sizeof(seamCijkSeen[d]));   /* ... so only the upload is left */
         if (MB200LaunchLogLikeForDivision (chain, d, &(m->lnLike[2*chain + state[chain]])) == NO)
             {
-            MrBayesPrint ("%s   B200 engine: division %d is outside the engine's coverage\n", spacer, d+1);
+            MrBayesPrint ("%s   H100 engine: division %d is outside the engine's coverage\n", spacer, d+1);
             m->lnLike[2*chain + state[chain]] = MRBFLT_NEG_MAX;
             abortMove = YES;
             }
@@ -2088,7 +2088,7 @@ static int SeamSyncHost (int division, int chain)
         rc = seamBackend.get_scalers (sd->instance, m->siteScalerIndex[chain], m->scalers[m->siteScalerIndex[chain]]);
     if (rc != MB200_SUCCESS)
         {
-        MrBayesPrint ("%s   B200 engine: cannot read the buffers of division %d back (%s)\n", spacer, division+1, mb200_error_string (rc));
+        MrBayesPrint ("%s   H100 engine: cannot read the buffers of division %d back (%s)\n", spacer, division+1, mb200_error_string (rc));
         return (ERROR);
         }
     sd->syncedStamp = sd->evalStamp; sd->syncedChain = chain; sd->syncedState = state[chain];

@@ -3,7 +3,7 @@
  *
  * The seam TU (mb200_seam.c) defines the mbbeagle.h entry points
  * (InitBeagleInstance, LaunchBEAGLELogLikeForDivision, TreeTiProbs_Beagle,
- * TreeCondLikes_Beagle_*, TreeLikelihood_Beagle) against the B200 engine; this
+ * TreeCondLikes_Beagle_*, TreeLikelihood_Beagle) against the H100 engine; this
  * header declares only the few extra symbols a caller needs.
  */
 #ifndef MB200_SEAM_H_

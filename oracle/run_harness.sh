@@ -12,7 +12,7 @@ BIN=oracle/_ref/mb_b200
 START=$(date +%s.%N)
 MB200_MODE=$MODE MB200_REPORT=$TMP/report.json timeout -s KILL ${MB200_TIMEOUT:-900} $BIN $TMP/run.nex > $TMP/run.log 2>$TMP/run.err || { tail -5 $TMP/run.log $TMP/run.err; exit 1; }
 END=$(date +%s.%N)
-grep -E "Using B200|Using standard|likelihood calculator" $TMP/run.log | head -3 || true
+grep -E "Using H100|Using standard|likelihood calculator" $TMP/run.log | head -3 || true
 head -5 $TMP/run.err || true
 python3 - "$TMP/report.json" "$START" "$END" "$STEM" "$NGEN" >> $REPORT <<'PY'
 import json, sys

@@ -1,5 +1,5 @@
 """Dev probe: wall time per evaluation of a small codon workload (replicase-sized: 61 states, 239
-patterns, 8 chains) -- the grid is far below one CTA per SM, i.e. the regime of the two-slot tcgen05 kernel.
+patterns, 8 chains) -- the grid is far below one CTA per SM, i.e. the regime of the tensor-core kernel.
 MB200_TC_ONE_SLOT=1 forces the one-slot variant."""
 import sys, time
 sys.path.insert(0, '/root/repo')

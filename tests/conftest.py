@@ -25,7 +25,7 @@ GOLDEN_FILES = [
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); run with -m gpu")
 
 
 @pytest.fixture(scope="session")
@@ -43,5 +43,5 @@ def engine_lib():
     device is an error, never a skip to a fallback."""
     from mrbayes_b200 import abi
     lib = abi.engine_library()
-    assert lib.fn("device_count")() >= 1, "no sm_100 device: the engine has no CPU fallback"
+    assert lib.fn("device_count")() >= 1, "no sm_90 device: the engine has no CPU fallback"
     return lib

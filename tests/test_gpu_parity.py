@@ -451,7 +451,7 @@ def test_variable_state_general_matrices(engine_lib, oracle_lib):
 
 
 def test_tensor_core_kernel_serves_20_and_61_states(engine_lib):
-    """S = 20 and S = 61 must run on the tcgen05 kernel, not on the CUDA-core correctness path
+    """S = 20 and S = 61 must run on the wgmma kernel, not on the CUDA-core correctness path
     (which would pass the same parity tolerance)."""
     for S, K in ((20, 4), (20, 1), (61, 1), (61, 3)):          # (61, 3): omega categories (NY98 / M3)
         pr = workloads.make_problem(S, K, 300, 8, 1, seed=3)

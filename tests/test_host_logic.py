@@ -33,7 +33,7 @@ def test_struct_sizes_match_the_header():
 
 
 def test_no_cpu_fallback_without_device():
-    """Without a B200 the engine must refuse, not compute somewhere else."""
+    """Without an H100 the engine must refuse, not compute somewhere else."""
     lib = abi.engine_library()
     if lib.fn("device_count")() > 0:
         pytest.skip("a device is present; covered by the gpu tests")

@@ -28,7 +28,18 @@ BIN = ROOT / "oracle" / "_ref" / "mb_b200"
 BIN_BATCHED = ROOT / "oracle" / "_ref" / "mb_b200_batched"     # the same objects with the patched RunChain (oracle/patch_runchain.py)
 CMD = ROOT / "tests" / "golden" / "cmd"
 
-needs_harness = pytest.mark.skipif(not BIN.exists(), reason="oracle/_ref/mb_b200 not built (needs /root/reference at build time)")
+needs_harness = pytest.mark.skipif(not BIN.exists(), reason="oracle/_ref/mb_b200 not built (needs the reference sources at build time)")
+
+
+def run_mb(binary: Path, nex: Path, env, timeout=900):
+    """Run a reference binary on the command file `nex` from the file's directory.  MrBayes keeps file names in
+    100-character buffers, so every path it sees is made relative to that directory (the example alignments through a
+    `data` link to oracle/_ref/data): a long checkout or temporary-directory path must not fail the run."""
+    d = nex.parent
+    if not (d / "data").exists():
+        (d / "data").symlink_to(ROOT / "oracle" / "_ref" / "data")
+    nex.write_text(nex.read_text().replace("oracle/_ref/data/", "data/").replace(str(d) + "/", ""))
+    return subprocess.run([str(binary), nex.name], cwd=d, env=env, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=timeout)
 
 
 def run_harness(tmp_path: Path, stem: str, ngen: int, mode: str, via: str = "seam", extra_env=None, timeout=900, binary: Path = BIN, tag: str = ""):
@@ -40,7 +51,7 @@ def run_harness(tmp_path: Path, stem: str, ngen: int, mode: str, via: str = "sea
     report = tmp_path / f"{key}.json"
     env = dict(os.environ, MB200_MODE=mode, MB200_REPORT=str(report), MB200_VIA=via)
     env.update(extra_env or {})
-    p = subprocess.run([str(binary), str(nex)], cwd=ROOT, env=env, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=timeout)
+    p = run_mb(binary, nex, env, timeout=timeout)
     assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-2000:]
     assert report.exists(), p.stdout[-2000:] + p.stderr[-2000:]
     rep = json.loads(report.read_text().strip().splitlines()[-1])
@@ -82,7 +93,7 @@ def test_function_pointer_forms_record_the_same_evaluations(tmp_path, stem, ngen
 # sample exactly what the unmodified reference samples: same accept / reject decisions, same trees, same lnL, every
 # generation.  (The reference's seed, proposals and acceptance draws are untouched: the acceptance variate is drawn
 # at the same position of the random stream.)
-needs_batched = pytest.mark.skipif(not BIN_BATCHED.exists(), reason="oracle/_ref/mb_b200_batched not built (needs /root/reference at build time)")
+needs_batched = pytest.mark.skipif(not BIN_BATCHED.exists(), reason="oracle/_ref/mb_b200_batched not built (needs the reference sources at build time)")
 
 
 @needs_harness
@@ -124,7 +135,7 @@ def _run_inline(tmp_path, binary, mode, data, cmds, ngen, tag, env=None):
     report = d / "r.json"
     e = dict(os.environ, MB200_MODE=mode, MB200_BATCH="1", MB200_REPORT=str(report))
     e.update(env or {})
-    p = subprocess.run([str(binary), str(nex)], cwd=ROOT, env=e, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=900)
+    p = run_mb(binary, nex, e, timeout=900)
     assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-2000:]
     rep = json.loads(report.read_text().strip().splitlines()[-1])
     rep["samples"] = {f.name: "\n".join(l for l in f.read_text().splitlines() if "ID:" not in l)
@@ -155,7 +166,7 @@ def test_chain_batched_generations_with_other_chain_layouts(tmp_path, mc):
                        f"mcmc {mc} printfreq=100000 samplefreq=25 diagnfreq=100000 filename={d}/o;\nquit;\n")
         report = d / "r.json"
         e = dict(os.environ, MB200_MODE=mode, MB200_BATCH="1", MB200_REPORT=str(report))
-        p = subprocess.run([str(binary), str(nex)], cwd=ROOT, env=e, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=900)
+        p = run_mb(binary, nex, e, timeout=900)
         assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-2000:]
         rep = json.loads(report.read_text().strip().splitlines()[-1])
         rep["samples"] = {f.name: "\n".join(l for l in f.read_text().splitlines() if "ID:" not in l)
@@ -183,7 +194,7 @@ def _run_printing(tmp_path, stem, ngen, env, tag, mode="oracle"):
     report = tmp_path / f"r{tag}.json"
     e = dict(os.environ, MB200_MODE=mode, MB200_BATCH="1", MB200_REPORT=str(report))
     e.update(env)
-    p = subprocess.run([str(BIN_BATCHED), str(nex)], cwd=ROOT, env=e, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=900)
+    p = run_mb(BIN_BATCHED, nex, e, timeout=900)
     assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-2000:]
     return json.loads(report.read_text().strip().splitlines()[-1]), _lnl_columns(p.stdout)
 
@@ -299,7 +310,7 @@ def _run_sweep_case(tmp_path, data, cmds, ngen, env):
     report = tmp_path / "sweep.json"
     e = dict(os.environ, MB200_MODE="shadow", MB200_REPORT=str(report))
     e.update(env)
-    p = subprocess.run([str(BIN_SCALAR), str(nex)], cwd=ROOT, env=e, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=900)
+    p = run_mb(BIN_SCALAR, nex, e, timeout=900)
     assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-2000:]
     return json.loads(report.read_text().strip().splitlines()[-1])
 
@@ -330,7 +341,7 @@ def _run_session(tmp_path, binary, mode, tag, env=None):
     report = d / "r.json"
     e = dict(os.environ, MB200_MODE=mode, MB200_BATCH="1", MB200_REPORT=str(report))
     e.update(env or {})
-    p = subprocess.run([str(binary), str(nex)], cwd=ROOT, env=e, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=900)
+    p = run_mb(binary, nex, e, timeout=900)
     assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-2000:]
     rep = json.loads(report.read_text().strip().splitlines()[-1])
     rep["samples"] = {f.name: "\n".join(l for l in f.read_text().splitlines() if "ID:" not in l)
@@ -390,7 +401,7 @@ def test_function_pointer_forms_drive_like_the_seam_loop_over_models(tmp_path, d
                        f"mcmc nruns=1 nchains=2 ngen=100 printfreq=100000 samplefreq=25 diagnfreq=100000 filename={d}/o;\nquit;\n")
         report = d / "r.json"
         e = dict(os.environ, MB200_MODE="oracle", MB200_VIA=via, MB200_MULTIPART="0", MB200_EIGEN="host", MB200_REPORT=str(report))
-        p = subprocess.run([str(BIN_SCALAR), str(nex)], cwd=ROOT, env=e, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=900)
+        p = run_mb(BIN_SCALAR, nex, e, timeout=900)
         assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-2000:]
         rep = json.loads(report.read_text().strip().splitlines()[-1])
         rep["samples"] = {f.name: "\n".join(l for l in f.read_text().splitlines() if "ID:" not in l)
@@ -575,7 +586,7 @@ def test_chain_batched_launches_equal_per_chain_launches_over_data_sets(tmp_path
         report = d / "r.json"
         e = dict(os.environ, MB200_MODE="gpu", MB200_BATCH=batch, MB200_REPORT=str(report))
         e.update(env)
-        p = subprocess.run([str(BIN_BATCHED), str(nex)], cwd=ROOT, env=e, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=900)
+        p = run_mb(BIN_BATCHED, nex, e, timeout=900)
         assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-2000:]
         rep = json.loads(report.read_text().strip().splitlines()[-1])
         rep["samples"] = {f.name: "\n".join(l for l in f.read_text().splitlines() if "ID:" not in l)
