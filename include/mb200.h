@@ -310,7 +310,10 @@ int mb200_replay           (int instance, int batch);
 int mb200_replay_results   (int instance, int batch, double *lnL, int *status);
 /* the same launch with the results delivered like mb200_evaluate_begin / _end delivers them (16-byte
  * records written by the kernel into pinned host memory, the caller polls): resident descriptors in,
- * lnL on the host out, no copy and no stream synchronisation.  One launch in flight per instance. */
+ * lnL on the host out, no copy and no stream synchronisation.  One launch in flight per instance.
+ * Small 4-state batches on an instance that is alone on its device are served by a kernel that stays
+ * resident on the instance's stream after mb200_replay_end returns: until the next other call on the
+ * instance, mb200_synchronize, or about 100 us without a new mb200_replay_begin. */
 int mb200_replay_begin     (int instance, int batch);
 int mb200_replay_end       (int instance, double *lnL, int *status);
 int mb200_free_batch       (int instance, int batch);

@@ -118,6 +118,23 @@ struct JobIndex
     JobIndexEntry e[MB200_JOB_INDEX_MAX];
 };
 
+// Resident generation kernel (mb200_replay_begin / _end): the host posts a job as 16-byte pieces in
+// pinned, mapped host memory, and every piece carries the job's sequence number in .w, so a reader
+// that finds the same number in every piece it read has an untorn job.
+//   piece 0: count (MB200_RES_STOP: exit), blob address lo, hi     piece 1: result address lo, hi, offEval
+//   piece 2: offDbl, offChunk, offCmat                             piece 3: offOp
+//   piece 4 + 2e, 5 + 2e: JobIndexEntry of evaluation e (matOff, nMat, opOff | nOp, dOff, eigen0)
+#define MB200_RES_HEAD   4
+#define MB200_RES_PIECES (MB200_RES_HEAD + 2 * MB200_JOB_INDEX_MAX)
+#define MB200_RES_STOP   0x7fffffff
+struct ResidentJob                  // device memory: the leader CTA's copy of the current job for the others
+{
+    unsigned long long word;        // sequence number << 32 | count (MB200_RES_STOP: exit)
+    unsigned int ack;               // jobs seen, summed over the CTAs (monotone, wraps)
+    unsigned int pad;
+    int4 piece[MB200_RES_PIECES];
+};
+
 // evaluations with at most this many pattern tiles add their tile partials left to right -- on the
 // device (last CTA) or, on the host-call latency path, on the host: the same order, the same bits
 #define MB200_SEQ_SUM_TILES 16

@@ -12,6 +12,7 @@
 #include "mb200_kernels_std.cuh"
 
 #include <cuda_runtime.h>
+#include <emmintrin.h>
 #include <float.h>
 #include <stdio.h>
 #include <time.h>
@@ -123,6 +124,15 @@ struct Instance
     bool          timing = false;      // bracket the fused kernel with events
     std::vector<cudaEvent_t> evA, evB; // ring of event pairs
     long long     evCount = 0;         // pairs recorded since the last read
+    // resident generation kernel (mb200_replay_begin / _end, eval_nuc4_resident_kernel)
+    int4         *hMail = nullptr;     // host -> device mailbox: pinned, mapped, MB200_RES_PIECES pieces
+    int4         *hMailDev = nullptr;  // its device alias
+    ResidentJob  *dJob = nullptr;      // the leader CTA's copy of the current job
+    int           resFits = -1;        // the grid fits the device at once (-1: not checked yet)
+    bool          resident = false;    // a resident kernel may still run on the stream
+    bool          pendingResident = false;   // the pending evaluation was posted to it
+    Batch        *resBatch = nullptr;  // what the pending post runs (a relaunch posts it again)
+    double        resPosted = 0.0;     // host clock (s) just before the last post
 };
 
 std::mutex               gLock;
@@ -167,10 +177,14 @@ Instance *get (int id)
     return gInstances[id];
 }
 
+int retire (Instance *I);
+
+// every entry point that touches the instance's stream or buffers comes through here: a resident
+// kernel is stopped and waited for first
 int use (Instance *I)
 {
     CK (cudaSetDevice (I->cfg.device));
-    return MB200_SUCCESS;
+    return retire (I);
 }
 
 int ensureStage (Instance *I, size_t bytes)
@@ -833,25 +847,195 @@ int launch (Instance *I, Batch &b, DevResult *res, bool viaParams, bool hostSum 
     return MB200_SUCCESS;
 }
 
-// wait until the kernel has written `slots` results into the mapped host buffer
+// ---- resident generation kernel (eval_nuc4_resident_kernel) ----------------------------------
+// A generation of the replay path costs a launch, the time until the kernel starts and the time until
+// its results reach the host, all on the critical path, because generation g+1 cannot start before
+// the host has read g's lnL.  Instead one kernel stays resident and the host posts each batch to a
+// mailbox in mapped host memory.
+const unsigned long long RES_IDLE_NS = 100000;   // the kernel exits by itself after this long without a job
+const double RES_DEADLINE_S = 10.0;              // longest host wait for the results of a posted job
+
+double wallNow () { struct timespec ts; clock_gettime (CLOCK_MONOTONIC, &ts); return (double) ts.tv_sec + 1e-9 * (double) ts.tv_nsec; }
+
+// write one post: every 16-byte piece carries the sequence number and is written by one aligned
+// 16-byte store, so the leader CTA sees each piece whole, from this post or from an earlier one
+void post (Instance *I, int seq, int count, const Batch *b)
+{
+    const int nP = MB200_RES_HEAD + 2 * I->maxEval;
+    alignas(16) int4 p[MB200_RES_PIECES];
+    memset (p, 0, sizeof(p));
+    p[0].x = count;
+    if (b)
+        {
+        const unsigned long long blob = (unsigned long long) b->dBlob, res = (unsigned long long) b->hResDev;
+        p[0].y = (int)(unsigned) blob; p[0].z = (int)(unsigned)(blob >> 32);
+        p[1].x = (int)(unsigned) res;  p[1].y = (int)(unsigned)(res >> 32); p[1].z = (int) b->offEval;
+        p[2].x = (int) b->offDbl; p[2].y = (int) b->offChunk; p[2].z = (int) b->offCmat;
+        p[3].x = (int) b->offOp;
+        for (int e = 0; e < b->nEval; e++)
+            {
+            const JobIndexEntry &je = b->jx.e[e];
+            p[MB200_RES_HEAD + 2*e]     = make_int4 (je.matOff, je.nMat, je.opOff, 0);
+            p[MB200_RES_HEAD + 2*e + 1] = make_int4 (je.nOp, je.dOff, je.eigen0, 0);
+            }
+        }
+    for (int i = 0; i < nP; i++)
+        {
+        p[i].w = seq;
+        _mm_store_si128 (reinterpret_cast<__m128i *>(I->hMail + i), _mm_load_si128 (reinterpret_cast<const __m128i *>(p + i)));
+        }
+    __atomic_signal_fence (__ATOMIC_SEQ_CST);
+}
+
+// K-dispatch of the resident kernel: with `go` false only checks that the whole grid fits the device
+// at once (every CTA must be running for a job to complete)
+template <int KK>
+int residentKernel (Instance *I, const DevCtx &ctx, dim3 grid, int seq0, bool go)
+{
+    auto kern = eval_nuc4_resident_kernel<KK, 256>;
+    constexpr int bytes = (int) sizeof(Nuc4Smem<KK, 256, true>);
+    if (!go)
+        {
+        int perSM = 0;
+        CK (cudaFuncSetAttribute (kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        CK (cudaOccupancyMaxActiveBlocksPerMultiprocessor (&perSM, kern, 256, bytes));
+        I->resFits = ((long) perSM * I->numSMs >= (long) grid.x * grid.y) ? 1 : 0;
+        return MB200_SUCCESS;
+        }
+    kern<<<grid, 256, bytes, I->stream>>> (ctx, I->hMailDev, I->dJob, seq0, RES_IDLE_NS);
+    CK (cudaGetLastError ());
+    return MB200_SUCCESS;
+}
+
+int residentDispatch (Instance *I, const DevCtx &ctx, dim3 grid, int seq0, bool go)
+{
+    switch (ctx.K)
+        {
+#define MB200_CASE(KK) case KK: return residentKernel<KK> (I, ctx, grid, seq0, go);
+        MB200_CASE(1) MB200_CASE(2) MB200_CASE(3) MB200_CASE(4) MB200_CASE(5) MB200_CASE(6) MB200_CASE(7) MB200_CASE(8)
+#undef MB200_CASE
+        default: return MB200_ERROR_UNSUPPORTED;
+        }
+}
+
+DevCtx residentCtx (const Instance *I)
+{
+    DevCtx ctx = I->ctx;
+    ctx.tilePatterns = nuc4PatternsPerBlock (ctx.K, true);
+    ctx.patternTiles = (ctx.C + ctx.tilePatterns - 1) / ctx.tilePatterns;
+    ctx.numTiles = ctx.patternTiles;
+    ctx.hostSum = 1;
+    return ctx;
+}
+
+// Which batches the resident kernel serves: fused 4-state batches whose evaluations all reach the root,
+// whose tile partials the host sums and whose job index covers every evaluation -- and only while this
+// instance is the only one on its device, so that idle resident CTAs never hold SMs other analyses
+// (many instances, or the partitions of one analysis) launch into.  Kernel timing and throughput mode
+// keep their launches.
+bool residentEligible (Instance *I, const Batch &b)
+{
+    static const bool off = getenv ("MB200_NO_RESIDENT") != nullptr;     // A/B switch: one launch per generation
+    const mb200_instance_config &c = I->cfg;
+    if (off || I->std || c.state_count != 4 || c.category_count > 8 || NT_SMALL != 256 || I->timing ||
+        (c.flags & MB200_CONFIG_THROUGHPUT) || !b.fused || !b.allRoot || b.nEval > MB200_JOB_INDEX_MAX || b.jx.n != b.nEval ||
+        I->maxEval > MB200_JOB_INDEX_MAX || I->resFits == 0)
+        return false;
+    const DevCtx ctx = residentCtx (I);
+    if (ctx.numTiles > HOSTSUM_MAX_TILES)
+        return false;
+    {
+    std::lock_guard<std::mutex> g (gLock);
+    int live = 0;
+    for (const Instance *J : gInstances)
+        if (J && J->cfg.device == c.device) live++;
+    if (live != 1)
+        return false;
+    }
+    if (I->resFits < 0)
+        {
+        if (cudaHostAlloc ((void **)&I->hMail, sizeof(int4) * MB200_RES_PIECES, cudaHostAllocMapped) != cudaSuccess ||
+            cudaHostGetDevicePointer ((void **)&I->hMailDev, I->hMail, 0) != cudaSuccess ||
+            cudaMalloc ((void **)&I->dJob, sizeof(ResidentJob)) != cudaSuccess ||
+            cudaMemset (I->dJob, 0, sizeof(ResidentJob)) != cudaSuccess ||
+            residentDispatch (I, ctx, dim3 (ctx.numTiles, I->maxEval), 0, false) != MB200_SUCCESS)
+            {
+            cudaGetLastError ();
+            I->resFits = 0;
+            return false;
+            }
+        memset (I->hMail, 0, sizeof(int4) * MB200_RES_PIECES);
+        }
+    return I->resFits == 1;
+}
+
+// post batch b, launching a resident kernel first when none is running
+int residentStart (Instance *I, Batch &b)
+{
+    if (b.needInv && !I->invMaskValid)
+        {
+        int rc = retire (I);                           // the mask kernel must not queue behind a resident kernel
+        if (rc == MB200_SUCCESS) rc = ensureInvMask (I);
+        if (rc != MB200_SUCCESS) return rc;
+        }
+    // past half the idle timeout the kernel may have exited: a cheap check saves a lost post
+    if (I->resident && wallNow () - I->resPosted > 0.5e-9 * (double) RES_IDLE_NS && cudaStreamQuery (I->stream) == cudaSuccess)
+        I->resident = false;
+    const DevCtx ctx = residentCtx (I);
+    // a new kernel starts past every sequence number an earlier kernel may have left in its job copy
+    const int seq0 = I->resident ? 0 : ++I->seq;
+    const int seq = ++I->seq;
+    I->resPosted = wallNow ();
+    post (I, seq, b.nEval, &b);
+    if (!I->resident)
+        {
+        int rc = residentDispatch (I, ctx, dim3 (ctx.numTiles, I->maxEval), seq0, true);
+        if (rc != MB200_SUCCESS) return rc;
+        I->resident = true;
+        I->launches++; I->launchKind[MB200_KERNEL_NUC4]++;
+        }
+    I->lastHostSum = 1; I->lastTiles = ctx.numTiles;
+    I->pendingSeq = seq; I->pendingResident = true; I->resBatch = &b;
+    return MB200_SUCCESS;
+}
+
+// wait until the kernel has written `slots` results into the mapped host buffer.  While a resident
+// kernel serves the instance the stream never goes idle, so the wait has a wall-clock deadline; an
+// idle stream then means the kernel exited on its timeout before its leader took the post, so no CTA
+// ran the job and it is posted again to a new kernel.
 int waitResults (Instance *I, Batch &b, int slots)
 {
-    const int seq = I->pendingSeq;     // the launch begin() issued, whatever else ran on the instance since
     volatile DevResult *r = b.hRes;
     unsigned long long spins = 0;
+    const double t0 = wallNow ();
     for (int e = 0; e < slots; e++)
         {
-        while (r[e].seq != seq)
+        // pendingSeq: the launch or post begin() issued, whatever else ran on the instance since
+        while (r[e].seq != I->pendingSeq)
             {
 #if defined(__x86_64__)
             __builtin_ia32_pause ();
 #endif
-            if ((++spins & 0xfffff) == 0)
+            if ((++spins & (I->resident ? 0x3fffu : 0xfffffu)) == 0)
                 {
                 cudaError_t q = cudaStreamQuery (I->stream);
                 if (q == cudaSuccess)
                     {
-                    if (r[e].seq == seq) break;
+                    if (r[e].seq == I->pendingSeq) break;
+                    if (I->resident && I->pendingResident)
+                        {
+                        for (int i = 0; i < slots; i++)
+                            if (r[i].seq == I->pendingSeq)
+                                {
+                                fprintf (stderr, "mb200: resident kernel exited in the middle of a job\n");
+                                return MB200_ERROR_GENERAL;
+                                }
+                        I->resident = false;
+                        int rc = residentStart (I, *I->resBatch);
+                        if (rc != MB200_SUCCESS) return rc;
+                        e = -1;                 // every slot again, for the new sequence number
+                        break;
+                        }
                     // stream idle but no result: treat as failure rather than spin forever
                     if (spins > (1ull << 26)) return MB200_ERROR_GENERAL;
                     }
@@ -860,11 +1044,33 @@ int waitResults (Instance *I, Batch &b, int slots)
                     fprintf (stderr, "mb200: CUDA error %s while waiting for results\n", cudaGetErrorName (q));
                     return MB200_ERROR_CUDA;
                     }
+                else if (I->resident && wallNow () - t0 > RES_DEADLINE_S)
+                    {
+                    fprintf (stderr, "mb200: no results from the resident kernel within %.0f s\n", RES_DEADLINE_S);
+                    return MB200_ERROR_GENERAL;
+                    }
                 }
             }
         }
     // the lnL / status words are ordinary loads: order them after the sequence-number polls
     __atomic_thread_fence (__ATOMIC_ACQUIRE);
+    return MB200_SUCCESS;
+}
+
+// stop the resident kernel (if any) and wait for it to exit; a job still pending is collected first,
+// so that the stop does not overwrite a post the leader has not taken yet
+int retire (Instance *I)
+{
+    if (!I->resident)
+        return MB200_SUCCESS;
+    if (I->pendingCount > 0 && I->pendingResident)
+        {
+        int rc = waitResults (I, *I->pendingBatch, I->pendingCount * I->lastTiles);
+        if (rc != MB200_SUCCESS) return rc;
+        }
+    I->resident = false;
+    post (I, ++I->seq, MB200_RES_STOP, nullptr);
+    CK (cudaStreamSynchronize (I->stream));     // bounded: the leader takes the stop within microseconds, or has exited
     return MB200_SUCCESS;
 }
 
@@ -893,7 +1099,7 @@ int runBegin (Instance *I, const mb200_evaluation *evs, int count)
     rc = launch (I, b, b.hResDev, viaParams, b.allRoot && b.fused);
     MB200_HOST_T (tC);
     if (rc != MB200_SUCCESS) return rc;
-    I->pendingCount = count; I->pendingBatch = &b; I->pendingSeq = I->seq;
+    I->pendingCount = count; I->pendingBatch = &b; I->pendingSeq = I->seq; I->pendingResident = false;
 #ifdef MB200_PHASE_TIMING
     gHostPhase[0] += tB - tA; gHostPhase[1] += tC - tB; gHostPhase[3] += 1.0;
 #endif
@@ -913,6 +1119,7 @@ int runEnd (Instance *I, double *lnL, int *status)
         {
         // results land in pinned host memory; no D2H copy, no stream synchronisation
         int rc = waitResults (I, b, I->lastHostSum ? count * I->lastTiles : count);
+        I->pendingResident = false;
         if (rc != MB200_SUCCESS) return rc;
         }
     else
@@ -969,6 +1176,7 @@ void destroy (Instance *I)
 {
     if (!I) return;
     cudaSetDevice (I->cfg.device);
+    retire (I);
     if (I->stream) cudaStreamSynchronize (I->stream);
     freeBatch (I->scratch);
     for (Batch *b : I->batches) if (b) { freeBatch (*b); delete b; }
@@ -984,6 +1192,8 @@ void destroy (Instance *I)
     for (cudaEvent_t e : I->evEigIn) cudaEventDestroy (e);
     if (I->hostStage) cudaFreeHost (I->hostStage);
     if (I->hMatRing) cudaFreeHost (I->hMatRing);
+    if (I->hMail) cudaFreeHost (I->hMail);
+    cudaFree (I->dJob);
     for (cudaEvent_t e : I->evMatRing) cudaEventDestroy (e);
     for (cudaEvent_t e : I->evA) cudaEventDestroy (e);
     for (cudaEvent_t e : I->evB) cudaEventDestroy (e);
@@ -1693,14 +1903,23 @@ int mb200_replay_begin (int instance, int batch)
     if (!I) return MB200_ERROR_BAD_INSTANCE;
     if (batch < 0 || batch >= (int) I->batches.size () || !I->batches[batch]) return MB200_ERROR_OUT_OF_RANGE;
     if (I->pendingCount > 0) return MB200_ERROR_OUT_OF_RANGE;       // one evaluation in flight per instance
-    int rc = use (I); if (rc) return rc;
+    CK (cudaSetDevice (I->cfg.device));                               // not use (): a resident kernel stays
     Batch &rb = *I->batches[batch];
     if (rb.tipEpoch != I->tipEpoch)
         return MB200_ERROR_OUT_OF_RANGE;
-    I->lastHostSum = 0; I->lastTiles = 1;
-    rc = launch (I, rb, rb.hResDev, false, rb.allRoot && rb.fused);
+    int rc;
+    if (residentEligible (I, rb))
+        rc = residentStart (I, rb);
+    else
+        {
+        rc = retire (I);
+        if (rc != MB200_SUCCESS) return rc;
+        I->lastHostSum = 0; I->lastTiles = 1;
+        rc = launch (I, rb, rb.hResDev, false, rb.allRoot && rb.fused);
+        I->pendingSeq = I->seq; I->pendingResident = false;
+        }
     if (rc != MB200_SUCCESS) return rc;
-    I->pendingCount = rb.nEval; I->pendingBatch = &rb; I->pendingSeq = I->seq;
+    I->pendingCount = rb.nEval; I->pendingBatch = &rb;
     return MB200_SUCCESS;
 }
 
@@ -1709,7 +1928,7 @@ int mb200_replay_end (int instance, double *lnL, int *status)
     Instance *I = get (instance);
     if (!I) return MB200_ERROR_BAD_INSTANCE;
     if (!lnL || !status) return MB200_ERROR_OUT_OF_RANGE;
-    int rc = use (I); if (rc) return rc;
+    CK (cudaSetDevice (I->cfg.device));
     return runEnd (I, lnL, status);
 }
 
