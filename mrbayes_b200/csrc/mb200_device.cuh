@@ -74,9 +74,7 @@ struct DevOp                        // one interior-node update (48 bytes)
 #define NUC_PRE      4u             // interior child this evaluation does not write, latency path: fetched into shared
                                     // memory when the chunk starts (slot in NucOp::pad), off the node chain
 #define NUC_FWD      8u             // the previous node's result: stays in registers
-#ifndef NUC_MAXPRE
 #define NUC_MAXPRE   8              // such operands per chunk
-#endif
 #define NUC_RESCALE  0x1000u
 struct NucOp
 {
@@ -90,21 +88,6 @@ struct NucOp
     int dest;
     int pad;                        // bits 4j..4j+3: shared-memory slot of operand j when its kind is NUC_PRE
 };
-// tip operands of a chunk get a 16-entry lookup table each (state mask -> P(t) column sum, per rate
-// category): tables per chunk, as a function of K (24 KB of shared memory)
-#ifdef MB200_STREAM4                // experiment: geometry that fits four 256-thread CTAs per SM
-#define NUC_MAXT(K) ((64 / (K)) > 64 ? 64 : (64 / (K)))
-#define NUC_OPC(PPB) ((1536 / (PPB) > 24) ? 24 : (1536 / (PPB) < 8 ? 8 : 1536 / (PPB)))
-#define NUC_STREAM_THREADS 1024
-#else
-#ifndef NUC_TABKB
-#define NUC_TABKB 96              // tip tables per chunk: NUC_TABKB / K (256 K bytes each)
-#endif
-#define NUC_MAXT(K) ((NUC_TABKB / (K)) > 64 ? 64 : (NUC_TABKB / (K)))
-#define NUC_OPC(PPB) ((2048 / (PPB) > 32) ? 32 : (2048 / (PPB) < 8 ? 8 : 2048 / (PPB)))   // nodes per chunk
-#define NUC_STREAM_THREADS 768      // resident threads per SM the streaming variant is compiled for
-#endif
-
 // Where the first chunk of each evaluation lives in the job blob, passed BY VALUE as a kernel
 // parameter: the 4-state kernel can then issue every staging load of a CTA (evaluation header,
 // branch list, node list, rates/frequencies, eigensystem) in one round instead of first fetching
@@ -139,28 +122,20 @@ struct ResidentJob                  // device memory: the leader CTA's copy of t
 // device (last CTA) or, on the host-call latency path, on the host: the same order, the same bits
 #define MB200_SEQ_SUM_TILES 16
 
-// chunk geometry of the 4-state kernels (shared by pack() and the kernels).  The latency-path (FUSE)
-// variants may be compiled with smaller shared-memory areas (-DNUC_FUSE_*) to fit more CTAs per SM.
-#ifndef NUC_FUSE_MAXS
-#define NUC_FUSE_MAXS 96
-#endif
-#ifndef NUC_FUSE_OPC
-#define NUC_FUSE_OPC 32
-#endif
-#ifndef NUC_FUSE_TABKB
-#define NUC_FUSE_TABKB NUC_TABKB
-#endif
-__host__ __device__ constexpr int nuc_maxs (int K, bool fuse)          // P(t) slots per chunk
+// chunk geometry of the 4-state kernels (shared by pack() and the kernels)
+__host__ __device__ constexpr int nuc_maxs (int K)          // P(t) slots per chunk
 {
-    return ((256 / K > 96) ? 96 : 256 / K) > (fuse ? NUC_FUSE_MAXS : 96) ? (fuse ? NUC_FUSE_MAXS : 96) : ((256 / K > 96) ? 96 : 256 / K);
+    return (256 / K > 96) ? 96 : 256 / K;
 }
-__host__ __device__ constexpr int nuc_opc (int ppb, bool fuse)         // nodes per chunk
+__host__ __device__ constexpr int nuc_opc (int ppb)         // nodes per chunk
 {
-    return (NUC_OPC (ppb) > (fuse ? NUC_FUSE_OPC : 32)) ? (fuse ? NUC_FUSE_OPC : 32) : NUC_OPC (ppb);
+    return (2048 / ppb > 32) ? 32 : (2048 / ppb < 8) ? 8 : 2048 / ppb;
 }
-__host__ __device__ constexpr int nuc_maxt (int K, bool fuse)          // tip operands (lookup tables) per chunk
+// tip operands of a chunk get a 16-entry lookup table each (state mask -> P(t) column sum, per rate
+// category, 256 K bytes): 96 / K tables per chunk (24 KB of shared memory), at most 64
+__host__ __device__ constexpr int nuc_maxt (int K)
 {
-    return (((fuse ? NUC_FUSE_TABKB : NUC_TABKB) / K) > 64) ? 64 : ((fuse ? NUC_FUSE_TABKB : NUC_TABKB) / K);
+    return (96 / K > 64) ? 64 : 96 / K;
 }
 
 struct DevResult                    // 16 bytes per evaluation
@@ -204,7 +179,6 @@ struct DevCtx                       // instance geometry + buffer bases, passed 
     double         *tilePartial;    // [maxEval][numTiles] per-tile lnL partial sums
     int            *tileAbort;      // [maxEval][numTiles]
     unsigned int   *ticket;         // [maxEval]
-    unsigned long long *dbg;        // [maxEval][64] phase timestamps (MB200_PHASE_TIMING builds only)
     int    cijkParts;               // eigensystems per cijk slot: 1, or K (category k uses part k: NY98-type models)
     int    patternTiles;            // 4-state path: tiles of tilePatterns patterns; numTiles (CTAs per evaluation) may be
                                     // smaller: a CTA then walks several tiles (throughput mode)

@@ -84,7 +84,6 @@ struct Instance
     double       *dTilePartial = nullptr;
     int          *dTileAbort = nullptr;
     unsigned int *dTicket = nullptr;
-    unsigned long long *dDbg = nullptr;
     bool          invMaskValid = false;
     int           maxEval = 1, maxTiles = 1, numSMs = 132;
     size_t        eigenStride = 0;     // doubles per eigen slot (all parts)
@@ -140,16 +139,7 @@ std::vector<Instance *>  gInstances;
 
 const int NT_GEN = 256;
 const int HOSTSUM_MAX_TILES = MB200_SEQ_SUM_TILES;   // latency path: up to this many tile partials per evaluation summed on the host
-// threads per CTA of the 4-state kernels: latency regime (FUSE) and bandwidth regime; both sizes are
-// compiled, MB200_NT_SMALL / MB200_NT_STREAM (128 or 256) pick at run time for tuning
-int ntFromEnv (const char *name, int dflt)
-{
-    const char *v = getenv (name);
-    int n = v ? atoi (v) : dflt;
-    return (n == 128 || n == 256) ? n : dflt;
-}
-const int NT_SMALL = ntFromEnv ("MB200_NT_SMALL", 256);
-const int NT_STREAM = ntFromEnv ("MB200_NT_STREAM", 256);
+const int NT_NUC4 = 256;                             // threads per CTA of the 4-state kernels
 const int EV_RING = 2048;
 
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { \
@@ -157,16 +147,10 @@ const int EV_RING = 2048;
     return MB200_ERROR_CUDA; } } while (0)
 
 // patterns one CTA of a 4-state kernel owns: NT threads / lanes-per-pattern (pow2ceil(K))
-int nuc4PatternsPerBlock (int K, bool small)
+int nuc4PatternsPerBlock (int K)
 {
     int L = (K <= 1) ? 1 : (K <= 2) ? 2 : (K <= 4) ? 4 : 8;
-    return (small ? NT_SMALL : NT_STREAM) / L;
-}
-
-int nuc4MinPatternsPerBlock (int K)
-{
-    int a = nuc4PatternsPerBlock (K, true), b = nuc4PatternsPerBlock (K, false);
-    return a < b ? a : b;
+    return NT_NUC4 / L;
 }
 
 Instance *get (int id)
@@ -252,23 +236,22 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
     const bool nuc4 = (S == 4 && K <= 8 && !I->std);
     // state frequencies per evaluation: S, or the whole table for variable-state divisions (one vector per state count)
     const int  nFreq = I->std ? MB200_MAX_STATES : S;
-    const int  ppbS = nuc4 ? nuc4PatternsPerBlock (K, true) : 1;
-    const long ctas = (long)((c.pattern_count + ppbS - 1) / ppbS) * count;
+    const int  ppb  = nuc4 ? nuc4PatternsPerBlock (K) : 1;
+    const long tiles = (c.pattern_count + ppb - 1) / ppb;
+    const long ctas = tiles * count;
     // fused P(t) rebuild (every CTA rebuilds the dirty matrices of its evaluation): small launches (latency-
     // bound regime), and launches of many evaluations over few pattern tiles each (the rebuild is repeated
     // only tiles-per-evaluation times, and a second kernel + its launch gap would cost more)
-    const long tilesS = (c.pattern_count + ppbS - 1) / ppbS;
-    const bool fused = nuc4 && (ctas <= 4L * I->numSMs || tilesS <= 16);
-    const int  ppb  = nuc4 ? nuc4PatternsPerBlock (K, fused) : 1;
-    const int  maxSlots = nuc_maxs (K > 0 ? K : 1, fused);      // as in the kernel
-    const int  opc = nuc_opc (ppb, fused);                      // nodes per chunk, as in the kernel
+    const bool fused = nuc4 && (ctas <= 4L * I->numSMs || tiles <= 16);
+    const int  maxSlots = nuc_maxs (K > 0 ? K : 1);             // as in the kernel
+    const int  opc = nuc_opc (ppb);                             // nodes per chunk, as in the kernel
     if ((int) I->slotOf.size () < c.matrix_count)
         { I->slotOf.assign (c.matrix_count, -1); I->dirtyOf.assign (c.matrix_count, -1); }
     std::vector<DevChunk> &chunks = I->chunkTmp;   // all evaluations, chunk0 of each included
     std::vector<DevMat>   &cmats  = I->cmatTmp;
     std::vector<int>      &slots  = I->slotTmp;    // 3 per operation
     std::vector<int>      &tipIdx = I->tipIdxTmp;  // 3 per operation: tip-table index within the chunk (-1: not a tip)
-    const int  maxTips = nuc_maxt (K > 0 ? K : 1, fused);
+    const int  maxTips = nuc_maxt (K > 0 ? K : 1);
     std::vector<int>      &nChunkOf = I->nChunkTmp;
     chunks.clear (); cmats.clear (); slots.clear (); tipIdx.clear (); nChunkOf.assign (count, 0);
 
@@ -657,52 +640,32 @@ int launchNuc4PK (Instance *I, const DevCtx &ctx, dim3 grid, const ParamBlob<CAP
     return MB200_SUCCESS;
 }
 
-template <int NT>
-int launchNuc4T (Instance *I, const DevCtx &ctx, dim3 grid, const DevEval *de, const double *dd, const DevChunk *dc,
-                 const DevMat *dm, const DevOp *dops, DevResult *res, int seq, bool fused, const JobIndex &jx)
-{
-    int rcl = MB200_SUCCESS;
-    switch (ctx.K)
-        {
-#define MB200_CASE(KK) case KK: rcl = fused ? launchNuc4K<KK, NT, true> (I, ctx, grid, de, dd, dc, dm, dops, res, seq, jx) \
-                                             : launchNuc4K<KK, NT, false> (I, ctx, grid, de, dd, dc, dm, dops, res, seq, jx); break;
-        MB200_CASE(1) MB200_CASE(2) MB200_CASE(3) MB200_CASE(4) MB200_CASE(5) MB200_CASE(6) MB200_CASE(7) MB200_CASE(8)
-#undef MB200_CASE
-        default: return MB200_ERROR_UNSUPPORTED;
-        }
-    return rcl;
-}
-
 int launchNuc4 (Instance *I, const DevCtx &ctx, dim3 grid, const DevEval *de, const double *dd, const DevChunk *dc,
                 const DevMat *dm, const DevOp *dops, DevResult *res, int seq, bool fused, const JobIndex &jx)
 {
-    const int nt = fused ? NT_SMALL : NT_STREAM;
-    return (nt == 256) ? launchNuc4T<256> (I, ctx, grid, de, dd, dc, dm, dops, res, seq, fused, jx)
-                       : launchNuc4T<128> (I, ctx, grid, de, dd, dc, dm, dops, res, seq, fused, jx);
-}
-
-// the same kernel with the job descriptors riding in the parameter block (no H2D copy)
-template <int CAP, int NT>
-int launchNuc4ParamT (Instance *I, const DevCtx &ctx, dim3 grid, const Batch &b, DevResult *res, int seq)
-{
-    const ParamBlob<CAP> &blob = *reinterpret_cast<const ParamBlob<CAP> *>(b.hBlob);
-    BlobOffsets off = { (int) b.offEval, (int) b.offDbl, (int) b.offUpd, (int) b.offChunk, (int) b.offCmat, (int) b.offOp };
-    int rcl = MB200_SUCCESS;
     switch (ctx.K)
         {
-#define MB200_CASE(KK) case KK: rcl = launchNuc4PK<KK, NT, CAP> (I, ctx, grid, blob, off, res, seq, b.jx); break;
+#define MB200_CASE(KK) case KK: return fused ? launchNuc4K<KK, NT_NUC4, true> (I, ctx, grid, de, dd, dc, dm, dops, res, seq, jx) \
+                                              : launchNuc4K<KK, NT_NUC4, false> (I, ctx, grid, de, dd, dc, dm, dops, res, seq, jx);
         MB200_CASE(1) MB200_CASE(2) MB200_CASE(3) MB200_CASE(4) MB200_CASE(5) MB200_CASE(6) MB200_CASE(7) MB200_CASE(8)
 #undef MB200_CASE
         default: return MB200_ERROR_UNSUPPORTED;
         }
-    return rcl;
 }
 
+// the same kernel with the job descriptors riding in the parameter block (no H2D copy)
 template <int CAP>
 int launchNuc4Param (Instance *I, const DevCtx &ctx, dim3 grid, const Batch &b, DevResult *res, int seq)
 {
-    return (NT_SMALL == 256) ? launchNuc4ParamT<CAP, 256> (I, ctx, grid, b, res, seq)
-                             : launchNuc4ParamT<CAP, 128> (I, ctx, grid, b, res, seq);
+    const ParamBlob<CAP> &blob = *reinterpret_cast<const ParamBlob<CAP> *>(b.hBlob);
+    BlobOffsets off = { (int) b.offEval, (int) b.offDbl, (int) b.offUpd, (int) b.offChunk, (int) b.offCmat, (int) b.offOp };
+    switch (ctx.K)
+        {
+#define MB200_CASE(KK) case KK: return launchNuc4PK<KK, NT_NUC4, CAP> (I, ctx, grid, blob, off, res, seq, b.jx);
+        MB200_CASE(1) MB200_CASE(2) MB200_CASE(3) MB200_CASE(4) MB200_CASE(5) MB200_CASE(6) MB200_CASE(7) MB200_CASE(8)
+#undef MB200_CASE
+        default: return MB200_ERROR_UNSUPPORTED;
+        }
 }
 
 const int PARAM_SMALL = 4096, PARAM_MID = 10240, PARAM_BIG = 30720;   // parameter-block sizes compiled (the launch copies all of it)
@@ -740,18 +703,12 @@ int launch (Instance *I, Batch &b, DevResult *res, bool viaParams, bool hostSum 
         }
     else if (b.nDirty > 0 && !b.fused)
         {
-        static const bool wideOld = getenv ("MB200_TIPROBS_WIDE") != nullptr;      // A/B switch: the c_ijk-streaming kernel
-        if (ctx.S > 32 && I->dFactor && !wideOld)
+        if (ctx.S > 32)             // dFactor is always allocated for these state counts
             {
             dim3 grid (b.nMat, ctx.K);
             const int LD = (ctx.S + 3) & ~3;
             tiprobs_mm_kernel<<<grid, 256, (size_t)2 * ctx.S * LD * sizeof(double), I->stream>>> (ctx, de, b.nEval, dd, du, I->dFactor,
                                                                                                    (I->tcS == 61) ? I->dSplit : nullptr);
-            }
-        else if (ctx.S > 32)
-            {
-            dim3 grid (b.nMat, ctx.K, (ctx.S + 3) / 4);
-            tiprobs_wide_kernel<<<grid, 128, 0, I->stream>>> (ctx, de, b.nEval, dd, du, (I->tcS == 61) ? I->dSplit : nullptr);
             }
         else
             {
@@ -780,7 +737,7 @@ int launch (Instance *I, Batch &b, DevResult *res, bool viaParams, bool hostSum 
         }
     else if (ctx.S == 4 && ctx.K <= 8)
         {
-        ctx.tilePatterns = nuc4PatternsPerBlock (ctx.K, b.fused);
+        ctx.tilePatterns = nuc4PatternsPerBlock (ctx.K);
         ctx.patternTiles = (ctx.C + ctx.tilePatterns - 1) / ctx.tilePatterns;
         ctx.numTiles = ctx.patternTiles;
         // throughput mode (MB200_CONFIG_THROUGHPUT): several analyses share the GPU, so SM time counts, not
@@ -806,12 +763,11 @@ int launch (Instance *I, Batch &b, DevResult *res, bool viaParams, bool hostSum 
     else if (I->tcS)
         {
         // tensor-core path: refresh the pre-split images of the matrices just rebuilt, then prune
-        // (61 states: tiprobs_wide_kernel has written them already)
+        // (61 states: tiprobs_mm_kernel has written them already)
         if (b.nDirty > 0 && I->tcS != 61)
             {
             dim3 sg (b.nMat, ctx.K);
-            if (I->tcS == 61) tc_split_kernel<61><<<sg, 128, 0, I->stream>>> (I->dMatrices, I->dSplit, du, 0, ctx.K);
-            else              tc_split_kernel<20><<<sg, 128, 0, I->stream>>> (I->dMatrices, I->dSplit, du, 0, ctx.K);
+            tc_split_kernel<20><<<sg, 128, 0, I->stream>>> (I->dMatrices, I->dSplit, du, 0, ctx.K);
             CK (cudaGetLastError ());
             I->launches++; I->launchKind[MB200_KERNEL_SETUP]++;
             }
@@ -892,17 +848,17 @@ void post (Instance *I, int seq, int count, const Batch *b)
 template <int KK>
 int residentKernel (Instance *I, const DevCtx &ctx, dim3 grid, int seq0, bool go)
 {
-    auto kern = eval_nuc4_resident_kernel<KK, 256>;
-    constexpr int bytes = (int) sizeof(Nuc4Smem<KK, 256, true>);
+    auto kern = eval_nuc4_resident_kernel<KK, NT_NUC4>;
+    constexpr int bytes = (int) sizeof(Nuc4Smem<KK, NT_NUC4, true>);
     if (!go)
         {
         int perSM = 0;
         CK (cudaFuncSetAttribute (kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-        CK (cudaOccupancyMaxActiveBlocksPerMultiprocessor (&perSM, kern, 256, bytes));
+        CK (cudaOccupancyMaxActiveBlocksPerMultiprocessor (&perSM, kern, NT_NUC4, bytes));
         I->resFits = ((long) perSM * I->numSMs >= (long) grid.x * grid.y) ? 1 : 0;
         return MB200_SUCCESS;
         }
-    kern<<<grid, 256, bytes, I->stream>>> (ctx, I->hMailDev, I->dJob, seq0, RES_IDLE_NS);
+    kern<<<grid, NT_NUC4, bytes, I->stream>>> (ctx, I->hMailDev, I->dJob, seq0, RES_IDLE_NS);
     CK (cudaGetLastError ());
     return MB200_SUCCESS;
 }
@@ -921,7 +877,7 @@ int residentDispatch (Instance *I, const DevCtx &ctx, dim3 grid, int seq0, bool 
 DevCtx residentCtx (const Instance *I)
 {
     DevCtx ctx = I->ctx;
-    ctx.tilePatterns = nuc4PatternsPerBlock (ctx.K, true);
+    ctx.tilePatterns = nuc4PatternsPerBlock (ctx.K);
     ctx.patternTiles = (ctx.C + ctx.tilePatterns - 1) / ctx.tilePatterns;
     ctx.numTiles = ctx.patternTiles;
     ctx.hostSum = 1;
@@ -935,9 +891,8 @@ DevCtx residentCtx (const Instance *I)
 // keep their launches.
 bool residentEligible (Instance *I, const Batch &b)
 {
-    static const bool off = getenv ("MB200_NO_RESIDENT") != nullptr;     // A/B switch: one launch per generation
     const mb200_instance_config &c = I->cfg;
-    if (off || I->std || c.state_count != 4 || c.category_count > 8 || NT_SMALL != 256 || I->timing ||
+    if (I->std || c.state_count != 4 || c.category_count > 8 || I->timing ||
         (c.flags & MB200_CONFIG_THROUGHPUT) || !b.fused || !b.allRoot || b.nEval > MB200_JOB_INDEX_MAX || b.jx.n != b.nEval ||
         I->maxEval > MB200_JOB_INDEX_MAX || I->resFits == 0)
         return false;
@@ -1074,35 +1029,21 @@ int retire (Instance *I)
     return MB200_SUCCESS;
 }
 
-#ifdef MB200_PHASE_TIMING
-static double hostNow () { struct timespec ts; clock_gettime (CLOCK_MONOTONIC, &ts); return ts.tv_sec * 1e6 + ts.tv_nsec * 1e-3; }
-double gHostPhase[4] = {0, 0, 0, 0};   // pack, launch, wait, calls
-#define MB200_HOST_T(var) const double var = hostNow ()
-#else
-#define MB200_HOST_T(var) do { } while (0)
-#endif
-
 // first half of an evaluation: validate, pack, launch.  Returns as soon as the work is queued.
 int runBegin (Instance *I, const mb200_evaluation *evs, int count)
 {
     if (I->pendingCount > 0)
         return MB200_ERROR_OUT_OF_RANGE;               // one evaluation in flight per instance
     Batch &b = I->scratch;
-    MB200_HOST_T (tA);
     int rc = pack (I, b, evs, count);
-    MB200_HOST_T (tB);
     if (rc != MB200_SUCCESS) return rc;
     const bool viaParams = paramEligible (I, b);
     if (!viaParams)
         CK (cudaMemcpyAsync (b.dBlob, b.hBlob, b.bytes, cudaMemcpyHostToDevice, I->stream));
     I->lastHostSum = 0; I->lastTiles = 1;
     rc = launch (I, b, b.hResDev, viaParams, b.allRoot && b.fused);
-    MB200_HOST_T (tC);
     if (rc != MB200_SUCCESS) return rc;
     I->pendingCount = count; I->pendingBatch = &b; I->pendingSeq = I->seq; I->pendingResident = false;
-#ifdef MB200_PHASE_TIMING
-    gHostPhase[0] += tB - tA; gHostPhase[1] += tC - tB; gHostPhase[3] += 1.0;
-#endif
     return MB200_SUCCESS;
 }
 
@@ -1114,7 +1055,6 @@ int runEnd (Instance *I, double *lnL, int *status)
         return MB200_ERROR_OUT_OF_RANGE;
     I->pendingCount = 0;
     Batch &b = *I->pendingBatch;
-    MB200_HOST_T (tC);
     if (b.allRoot)
         {
         // results land in pinned host memory; no D2H copy, no stream synchronisation
@@ -1124,9 +1064,6 @@ int runEnd (Instance *I, double *lnL, int *status)
         }
     else
         CK (cudaStreamSynchronize (I->stream));
-#ifdef MB200_PHASE_TIMING
-    { const double tD = hostNow (); gHostPhase[2] += tD - tC; }
-#endif
     for (int e = 0; e < count; e++)
         {
         if (b.hasRoot[e])
@@ -1182,7 +1119,7 @@ void destroy (Instance *I)
     for (Batch *b : I->batches) if (b) { freeBatch (*b); delete b; }
     cudaFree (I->dTip8); cudaFree (I->dTip64); cudaFree (I->dTipPartAmbig); cudaFree (I->dSplit); cudaFree (I->dPartials); cudaFree (I->dMatrices);
     cudaFree (I->dScalers); cudaFree (I->dWeights); cudaFree (I->dEigen); cudaFree (I->dFactor); cudaFree (I->dInvMask);
-    cudaFree (I->dTilePartial); cudaFree (I->dTileAbort); cudaFree (I->dTicket); cudaFree (I->dDbg);
+    cudaFree (I->dTilePartial); cudaFree (I->dTileAbort); cudaFree (I->dTicket);
     cudaFree (I->dStdTab); cudaFree (I->dStdClasses); cudaFree (I->dTilePartial2);
     cudaFree (I->dTcCounter); cudaFree (I->dTcFlags); cudaFree (I->dTcError);
     cudaFree (I->dEigIn); if (I->dEigVec != I->dFactor) cudaFree (I->dEigVec);
@@ -1287,7 +1224,7 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
     const bool nuc4 = (S == 4 && K <= 8 && !I->std);
     if (nuc4 && (nInt * K * C >= (1ull << 32) || (size_t)cfg->tip_count * C >= (1ull << 32)))
         { delete I; return MB200_ERROR_OUT_OF_RANGE; }      // 4-state records carry 32-bit element offsets (64 GB of partials)
-    if (!getenv ("MB200_DISABLE_TC") && !I->std)
+    if (!I->std)
         {
         if (S == 61 && K <= 3) I->tcS = 61;      // 61-state codon (K > 1: omega categories, NY98 / M3), wgmma path
         if (S == 20 && K <= 4) I->tcS = 20;      // 20-state amino acids, wgmma path
@@ -1297,7 +1234,7 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
     if (I->std)
         I->maxTiles = (C + 128 / stdLanes - 1) / (128 / stdLanes);
     else
-    I->maxTiles = I->tcS ? (C + TC_MIN_ROWS - 1) / TC_MIN_ROWS + 1 : nuc4 ? (C + nuc4MinPatternsPerBlock (K) - 1) / nuc4MinPatternsPerBlock (K) : (C + TP - 1) / TP;
+    I->maxTiles = I->tcS ? (C + TC_MIN_ROWS - 1) / TC_MIN_ROWS + 1 : nuc4 ? (C + nuc4PatternsPerBlock (K) - 1) / nuc4PatternsPerBlock (K) : (C + TP - 1) / TP;
 
 #define ALLOC(ptr, bytes) do { cudaError_t e_ = cudaMalloc ((void **)&(ptr), (bytes)); if (e_ != cudaSuccess) { \
         cudaGetLastError (); destroy (I); return (e_ == cudaErrorMemoryAllocation) ? MB200_ERROR_OUT_OF_MEMORY : MB200_ERROR_CUDA; } } while (0)
@@ -1356,7 +1293,6 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
     ALLOC (I->dTilePartial, (size_t)I->maxEval * I->maxTiles * sizeof(double));
     ALLOC (I->dTileAbort,   (size_t)I->maxEval * I->maxTiles * sizeof(int));
     ALLOC (I->dTicket,      (size_t)I->maxEval * sizeof(unsigned int));
-    ALLOC (I->dDbg,         ((size_t)I->maxEval * 64 + 4096) * sizeof(unsigned long long));
     if (I->std)
         {
         ALLOC (I->dStdTab,       (size_t)3 * C * sizeof(int));
@@ -1389,13 +1325,13 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
     x.S = S; x.Sp = Sp; x.K = K; x.C = C;
     x.tipCount = cfg->tip_count; x.partialsCount = cfg->partials_count; x.matrixCount = cfg->matrix_count;
     x.scalerCount = cfg->scaler_count; x.eigenCount = cfg->eigen_count; x.weightRows = cfg->weight_rows;
-    x.tilePatterns = I->tcS ? 128 : nuc4 ? nuc4PatternsPerBlock (K, false) : TP;
+    x.tilePatterns = I->tcS ? 128 : nuc4 ? nuc4PatternsPerBlock (K) : TP;
     x.genKB = KB;
     x.numTiles = I->maxTiles;
     x.tip8 = I->dTip8; x.tip64 = I->dTip64; x.tipPartAmbig = I->dTipPartAmbig; x.partials = I->dPartials; x.matrices = I->dMatrices;
     x.scalers = I->dScalers; x.eigen = I->dEigen; x.weights = I->dWeights; x.invMask = I->dInvMask;
     x.cijkParts = I->cijkParts; x.patternTiles = 0;
-    x.tilePartial = I->dTilePartial; x.tileAbort = I->dTileAbort; x.ticket = I->dTicket; x.dbg = I->dDbg;
+    x.tilePartial = I->dTilePartial; x.tileAbort = I->dTileAbort; x.ticket = I->dTicket;
 
     if (cudaStreamSynchronize (I->stream) != cudaSuccess) { destroy (I); return MB200_ERROR_CUDA; }
 
@@ -1603,10 +1539,9 @@ int mb200_set_rate_matrices (int instance, int eigen, int like_eigen, const doub
     int *dStatus = nullptr;
     CK (cudaHostGetDevicePointer ((void **)&dStatus, I->hEigStatus, 0));
     // warm start from the eigenvectors of a nearby matrix, unless that would extend an already long chain of warm starts
-    static const bool noWarm = getenv ("MB200_EIGEN_COLD") != nullptr;
     const double *U0 = nullptr;
     int chain = 0;
-    if (!noWarm && like_eigen >= 0 && like_eigen != eigen && I->eigWarmChain[like_eigen] >= 0 && I->eigWarmChain[like_eigen] < MB200_EIG_WARM_CHAIN)
+    if (like_eigen >= 0 && like_eigen != eigen && I->eigWarmChain[like_eigen] >= 0 && I->eigWarmChain[like_eigen] < MB200_EIG_WARM_CHAIN)
         {
         U0 = I->dEigU + (size_t)like_eigen * uLen;
         chain = I->eigWarmChain[like_eigen] + 1;
@@ -1993,36 +1928,6 @@ int mb200_get_kernel_launches (int instance, int kind, long long *launches)
     if (!I || !launches) return MB200_ERROR_BAD_INSTANCE;
     if (kind < 0 || kind >= MB200_KERNEL_KINDS) return MB200_ERROR_OUT_OF_RANGE;
     *launches = I->launchKind[kind];
-    return MB200_SUCCESS;
-}
-
-#ifdef MB200_PHASE_TIMING
-extern "C" int mb200_debug_host_phases (double *out4) { for (int i = 0; i < 4; i++) { out4[i] = gHostPhase[i]; gHostPhase[i] = 0; } return 0; }
-#endif
-
-// phase timestamps of the last launch (debug builds compiled with -DMB200_PHASE_TIMING only)
-int mb200_debug_read_stamps (int instance, unsigned long long *out, int evaluations)
-{
-    Instance *I = get (instance);
-    if (!I || !out) return MB200_ERROR_BAD_INSTANCE;
-    if (evaluations < 1 || evaluations > I->maxEval) return MB200_ERROR_OUT_OF_RANGE;
-    int rc = use (I); if (rc) return rc;
-    CK (cudaStreamSynchronize (I->stream));
-    CK (cudaMemcpy (out, I->dDbg, (size_t)evaluations * 64 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    CK (cudaMemset (I->dDbg, 0, (size_t)I->maxEval * 64 * sizeof(unsigned long long)));
-    return MB200_SUCCESS;
-}
-
-// pipeline trace of the tensor-core kernel's first CTA (debug builds only): 16 stamps per work item
-int mb200_debug_read_trace (int instance, unsigned long long *out, int count)
-{
-    Instance *I = get (instance);
-    if (!I || !out) return MB200_ERROR_BAD_INSTANCE;
-    if (count < 1 || count > 4096) return MB200_ERROR_OUT_OF_RANGE;
-    int rc = use (I); if (rc) return rc;
-    CK (cudaStreamSynchronize (I->stream));
-    CK (cudaMemcpy (out, I->dDbg, (size_t)count * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    CK (cudaMemset (I->dDbg, 0, ((size_t)I->maxEval * 64 + 4096) * sizeof(unsigned long long)));
     return MB200_SUCCESS;
 }
 

@@ -73,9 +73,6 @@ template <int S> inline int tcp_stages (int K, size_t limit)
     return (int) n;
 }
 
-#ifndef TCP_BACKOFF_NS
-#define TCP_BACKOFF_NS 32
-#endif
 // mbarrier wait that cannot hang the device: a CTA whose pipeline stalls for two seconds traps (the launch fails
 // with an error instead of sitting on the GPU until somebody's watchdog fires)
 __device__ __forceinline__ void tcp_wait (uint64_t *bar, uint32_t parity)
@@ -89,9 +86,7 @@ __device__ __forceinline__ void tcp_wait (uint64_t *bar, uint32_t parity)
                       "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
                       "selp.u32 %0, 1, 0, p;\n\t}\n" : "=r"(done) : "r"(a), "r"(parity) : "memory");
         if (done) return;
-#ifndef TCP_NO_BACKOFF
-        __nanosleep (TCP_BACKOFF_NS);          // a waiting warp must not compete for issue slots with the working ones
-#endif
+        __nanosleep (32);                      // a waiting warp must not compete for issue slots with the working ones
         if ((it & 0xfffu) == 0xfffu)
             {
             unsigned long long now;
@@ -108,16 +103,6 @@ __device__ __forceinline__ void tcp_bar_group (int grp)
     if (grp == 0) asm volatile ("bar.sync 1, 128;\n" ::: "memory");
     else          asm volatile ("bar.sync 2, 128;\n" ::: "memory");
 }
-
-// debug builds (-DMB200_PHASE_TIMING): CTA 0 stamps the pipeline events of its first items, 16 slots per item
-#ifdef MB200_PHASE_TIMING
-#define TCP_TRACE_ITEMS 250
-#define TCP_T(n, slot) do { if (blockIdx.x == 0 && (n) < TCP_TRACE_ITEMS) ctx.dbg[(n) * 16 + (slot)] = mb200_now (); } while (0)
-#define TCP_TV(n, slot, v) do { if (blockIdx.x == 0 && (n) < TCP_TRACE_ITEMS) ctx.dbg[(n) * 16 + (slot)] = (unsigned long long)(v); } while (0)
-#else
-#define TCP_T(n, slot) do { } while (0)
-#define TCP_TV(n, slot, v) do { } while (0)
-#endif
 
 template <int S>
 __global__ void __launch_bounds__(TCP_THREADS, 1)
@@ -166,11 +151,9 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
         {
         // =================================================================== scheduler
         int slot = 0; uint32_t ph = 0;
-        unsigned nItem = 0;
         for (;;)
             {
             tcp_wait (&barInfoEmpty[slot], ph ^ 1);
-            if (lane == 0) TCP_T (nItem, 1);
             int item = 0;
             if (lane == 0) item = (int)(atomicAdd (Q.counter, 1u) - Q.base);
             item = __shfl_sync (0xffffffffu, item, 0);
@@ -195,7 +178,6 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                     it.shortcut = (ev->flags & MB200_SHORTCUT_FLAG) ? 1 : 0;
                     it.child[0] = op.c1; it.child[1] = op.c2; it.child[2] = op.c3;
                     it.mat[0] = op.m1; it.mat[1] = op.m2; it.mat[2] = op.m3;
-                    if (lane == 0) TCP_T (nItem, 2);
                     if (lane < 3)
                         {
                         const int pr = (lane == 0) ? op.s1 : (lane == 1) ? op.s2 : op.s3;
@@ -231,10 +213,7 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                 {
                 sInfo[slot] = it;
                 mbar_arrive (&barInfoFull[slot]);              // release: the record is visible to whoever acquires the phase
-                TCP_TV (nItem, 0, (unsigned long long) it.kind | ((unsigned long long) it.t << 8) | ((unsigned long long) it.oi << 32));
-                TCP_T (nItem, 3);
                 }
-            nItem++;
             if (it.kind == TCP_ITEM_STOP)
                 break;
             if (++slot == TCP_NI) { slot = 0; ph ^= 1; }
@@ -252,7 +231,6 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
         const uint64_t fullMaskL = (S == 64) ? ~(uint64_t)0 : ((((uint64_t)1) << S) - 1);
         int islot = 0; uint32_t iph = 0;
         unsigned u = 0;                                         // units since the kernel started (all roles count alike)
-        unsigned nItem = 0;
         for (;;)
             {
             tcp_wait (&barInfoFull[islot], iph);
@@ -263,9 +241,8 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
             if (lane == 0) mbar_arrive (&barInfoEmpty[islot]);
             if (++islot == TCP_NI) { islot = 0; iph ^= 1; }
             if (kind == TCP_ITEM_STOP) break;
-            if (kind == TCP_ITEM_CLOSE) { nItem++; continue; }
+            if (kind == TCP_ITEM_CLOSE) continue;
             const int c0 = tileIdx * rows, np = min (rows, C - c0);
-            bool firstUnit = true;
             for (int k = 0; k < K; k++)
                 for (int ch = 0; ch < nChild; ch++, u++)
                     {
@@ -305,9 +282,6 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                             }
                         }
                     tcp_wait (&barEmpty[s], ph ^ 1);
-#ifndef TCP_TRACE_EPI
-                    if (ltid == 0 && firstUnit && grp < 2) TCP_T (nItem, 4 + 2 * grp);
-#endif
                     if (ltid == 0)
                         {
                         mbar_expect_tx (&barFull[s], (uint32_t)(B_FLOATS * 4));
@@ -352,12 +326,7 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                     fence_async_smem ();                        // generic-proxy stores -> async proxy (wgmma)
                     __syncwarp ();
                     if (lane == 0) mbar_arrive (&barFull[s]);
-#ifndef TCP_TRACE_EPI
-                    if (ltid == 0 && firstUnit && grp < 2) TCP_T (nItem, 5 + 2 * grp);
-#endif
-                    firstUnit = false;
                     }
-            nItem++;
             }
         }
     else if (warp == 17)
@@ -393,11 +362,9 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
         int islot = 0; uint32_t iph = 0;
         int pslot = 0; uint32_t pph = 0;
         unsigned u = 0;
-        unsigned nItem = 0;
-        for (;; nItem++)
+        for (;;)
             {
             tcp_wait (&barInfoFull[islot], iph);
-            if (tid == 0) TCP_T (nItem, 11);
             struct { int kind, e, t, oi, nChild, dest, sw, shortcut; } it;
             it.kind = sInfo[islot].kind; it.e = sInfo[islot].e; it.t = sInfo[islot].t; it.oi = sInfo[islot].oi;
             it.nChild = sInfo[islot].nChild; it.dest = sInfo[islot].dest; it.sw = sInfo[islot].sw; it.shortcut = sInfo[islot].shortcut;
@@ -431,7 +398,6 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                         const int child = (ch == 0) ? ch0 : (ch == 1) ? ch1 : ch2;
                         const bool isTip = child < ctx.tipCount;
                         tcp_wait (&barFull[s], (u / (unsigned) NS) & 1u);   // operand images (generic stores + bulk copy) have landed
-                        if (tid == 0 && k == 0 && ch == 0) TCP_T (nItem, 8);
                         const uint32_t st = smem_u32 (tcp_smem + (size_t) s * STAGE);
                         const uint64_t aHi = make_desc (st + grp * (64 / 8) * 128, LBO_A, SBO), aLo = aHi + A_LO;
                         const uint64_t bb  = make_desc (st + 2 * A_FLOATS * 4, LBO_B, SBO);
@@ -461,7 +427,6 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                             }
                         __syncwarp ();
                         if (lane == 0) mbar_arrive (&barEmpty[s]);     // operands read: the stage goes back to the loaders
-                        if (tid == 0 && k == K - 1 && ch == it.nChild - 1) TCP_T (nItem, 12);
                         const bool last = ch == it.nChild - 1;
                         #pragma unroll
                         for (int j = 0; j < NP / 8; j++)
@@ -498,7 +463,6 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                     mx[h] = fmaxf (mx[h], __shfl_xor_sync (0xffffffffu, mx[h], 2));
                     }
                 if ((lane & 3) == 0) { sMax[fRow] = mx[0]; sMax[fRow + 8] = mx[1]; }
-                if (tid == 0) TCP_T (nItem, 13);
                 // the warpgroups meet: row maxima, then the copy-out
                 tcp_bar_epilogue ();
                 const bool doScale = it.sw >= 0;
@@ -543,7 +507,6 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                 // publish: the barrier orders every epilogue thread's stores before thread 0's hand-over; the publisher warp
                 // acquires it and release-stores the flag (cumulative at GPU scope), so no epilogue warp sits in a memory
                 // barrier while the next item's accumulators are waiting
-                if (tid == 0) TCP_T (nItem, 14);
                 tcp_bar_epilogue ();
                 if (tid == 0)
                     {
@@ -551,7 +514,6 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                     sPub[pslot] = flagRow + it.oi;
                     mbar_arrive (&barPubFull[pslot]);
                     if (++pslot == TCP_NPUB) { pslot = 0; pph ^= 1; }
-                    TCP_T (nItem, 15);
                     }
                 continue;
                 }
