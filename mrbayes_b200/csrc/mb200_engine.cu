@@ -19,6 +19,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <mutex>
+#include <type_traits>
 #include <vector>
 
 namespace {
@@ -41,11 +42,20 @@ struct Batch                       // packed evaluations (device job format)
     bool    fused = false;         // 4-state latency path: P(t) rebuilt inside the pruning kernel
     bool    needInv = false;
     bool    singleChunk = false;   // every evaluation of the batch fits one chunk (4-state path)
-    bool    used = false;
     int     tipEpoch = 0;          // Instance::tipEpoch at pack time (4-state records embed tip kinds)
     JobIndex jx;                   // 4-state latency path: where each evaluation's first chunk lives
     std::vector<char> hasRoot;     // [nEval] the evaluation ends in a root integration
     bool    allRoot = false;
+};
+
+struct Pending                     // the evaluation begin() started and end() has not collected yet
+{
+    int     count = 0;             // evaluations (0: nothing pending)
+    int     seq = 0;               // sequence number the launch or post stamps into the results
+    Batch  *batch = nullptr;       // whose mapped result buffer it writes
+    bool    resident = false;      // posted to the resident kernel
+    bool    hostSum = false;       // every tile writes its partial lnL, the host adds them up
+    int     tiles = 1;             // tiles per evaluation (host sum only)
 };
 
 struct Instance
@@ -89,15 +99,11 @@ struct Instance
     size_t        eigenStride = 0;     // doubles per eigen slot (all parts)
     int           cijkParts = 1;       // eigensystems per slot (one per category for NY98-type models)
     size_t        smemGen = 0;         // dynamic smem of eval_gen_kernel
-    long long     launches = 0;
     long long     launchKind[MB200_KERNEL_KINDS] = {0};   // per kernel family (mb200_get_kernel_launches)
     std::vector<int> tipPartAmbig;  // host copy (operand kinds of the 4-state records)
     int           tipEpoch = 0;
     int           writtenStamp = 0;
-    int           pendingCount = 0;            // evaluations started by mb200_evaluate_begin, not yet collected
-    int           pendingSeq = 0;              // sequence number stamped by the launch begin() issued
-    Batch        *pendingBatch = nullptr;      // whose result buffer the pending launch writes
-    int           lastHostSum = 0, lastTiles = 1;   // how the last launch delivers its results
+    Pending       pending;
     Batch         scratch;             // used by the synchronous entry points
     std::vector<Batch *> batches;      // resident batches (mb200_pack_evaluations)
     void         *hostStage = nullptr; // pinned staging for set/get calls
@@ -127,10 +133,9 @@ struct Instance
     int4         *hMail = nullptr;     // host -> device mailbox: pinned, mapped, MB200_RES_PIECES pieces
     int4         *hMailDev = nullptr;  // its device alias
     ResidentJob  *dJob = nullptr;      // the leader CTA's copy of the current job
-    int           resFits = -1;        // the grid fits the device at once (-1: not checked yet)
+    bool          resOk = false;       // the resident kernel may serve this instance: 4-state, its grid fits the
+                                       // device at once, and (once tried) its mailbox could be allocated
     bool          resident = false;    // a resident kernel may still run on the stream
-    bool          pendingResident = false;   // the pending evaluation was posted to it
-    Batch        *resBatch = nullptr;  // what the pending post runs (a relaunch posts it again)
     double        resPosted = 0.0;     // host clock (s) just before the last post
 };
 
@@ -151,6 +156,24 @@ int nuc4PatternsPerBlock (int K)
 {
     int L = (K <= 1) ? 1 : (K <= 2) ? 2 : (K <= 4) ? 4 : 8;
     return NT_NUC4 / L;
+}
+
+// The 4-state kernels are compiled for K = 1..8 rate categories: calls f (std::integral_constant<int, K> ())
+template <int KK = 1, class F>
+int withNuc4K (int K, F &&f)
+{
+    if constexpr (KK > 8) return MB200_ERROR_UNSUPPORTED;
+    else return (K == KK) ? f (std::integral_constant<int, KK> ()) : withNuc4K<KK + 1> (K, f);
+}
+
+// dynamic shared memory of a 4-state kernel (the parameter-block and resident kernels take the fused layout)
+template <int K, bool FUSE> constexpr int nuc4Smem = (int) sizeof(Nuc4Smem<K, NT_NUC4, FUSE>);
+
+// The tensor-core kernels are compiled for S = 20 and 61 states: calls f (std::integral_constant<int, tcS> ())
+template <class F>
+auto withTcS (int tcS, F &&f)
+{
+    return (tcS == 61) ? f (std::integral_constant<int, 61> ()) : f (std::integral_constant<int, 20> ());
 }
 
 Instance *get (int id)
@@ -223,42 +246,20 @@ bool okPartials (const Instance *I, int b, bool allowTip)
     return b >= (allowTip ? 0 : I->cfg.tip_count) && b < I->cfg.partials_count;
 }
 
-// validate + flatten host evaluations into the device job format
-int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
+// ---- pack(): host evaluations -> device job format ---------------------------------------------
+// One blob per batch: DevBatchHeader | DevEval[nEval] | double[nDbl] | DevMat updates[] | DevChunk[] (chunks
+// after each evaluation's first) | DevMat chunk branches[] | records[nOp] | int order[nOp] (tensor-core path),
+// each section 16-byte aligned.  The 4-state family's records are NucOps, every other family's DevOps.
+
+// every count, pointer and index of the evaluations against the instance
+int validate (const Instance *I, const mb200_evaluation *evs, int count)
 {
     const mb200_instance_config &c = I->cfg;
-    const int K = c.category_count, S = c.state_count;
     if (count < 1 || count > I->maxEval)
         return MB200_ERROR_OUT_OF_RANGE;
     if (I->std && !I->stdReady)
         return MB200_ERROR_UNSUPPORTED;                 // mb200_set_pattern_states first
-
-    const bool nuc4 = (S == 4 && K <= 8 && !I->std);
-    // state frequencies per evaluation: S, or the whole table for variable-state divisions (one vector per state count)
-    const int  nFreq = I->std ? MB200_MAX_STATES : S;
-    const int  ppb  = nuc4 ? nuc4PatternsPerBlock (K) : 1;
-    const long tiles = (c.pattern_count + ppb - 1) / ppb;
-    const long ctas = tiles * count;
-    // fused P(t) rebuild (every CTA rebuilds the dirty matrices of its evaluation): small launches (latency-
-    // bound regime), and launches of many evaluations over few pattern tiles each (the rebuild is repeated
-    // only tiles-per-evaluation times, and a second kernel + its launch gap would cost more)
-    const bool fused = nuc4 && (ctas <= 4L * I->numSMs || tiles <= 16);
-    const int  maxSlots = nuc_maxs (K > 0 ? K : 1);             // as in the kernel
-    const int  opc = nuc_opc (ppb);                             // nodes per chunk, as in the kernel
-    if ((int) I->slotOf.size () < c.matrix_count)
-        { I->slotOf.assign (c.matrix_count, -1); I->dirtyOf.assign (c.matrix_count, -1); }
-    std::vector<DevChunk> &chunks = I->chunkTmp;   // all evaluations, chunk0 of each included
-    std::vector<DevMat>   &cmats  = I->cmatTmp;
-    std::vector<int>      &slots  = I->slotTmp;    // 3 per operation
-    std::vector<int>      &tipIdx = I->tipIdxTmp;  // 3 per operation: tip-table index within the chunk (-1: not a tip)
-    const int  maxTips = nuc_maxt (K > 0 ? K : 1);
-    std::vector<int>      &nChunkOf = I->nChunkTmp;
-    chunks.clear (); cmats.clear (); slots.clear (); tipIdx.clear (); nChunkOf.assign (count, 0);
-
-    // ---- pass 1: validate; 4-state path: cut every operation list into chunks whose branches fit
-    //      the kernel's shared-memory P(t) slots ----
-    int nMat = 0, nOp = 0, rcv = MB200_SUCCESS;
-    for (int e = 0; e < count && rcv == MB200_SUCCESS; e++)
+    for (int e = 0; e < count; e++)
         {
         const mb200_evaluation &ev = evs[e];
         if (ev.matrix_update_count < 0 || ev.operation_count < 0 ||
@@ -274,102 +275,235 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
             const mb200_matrix_update &u = ev.matrix_updates[i];
             const bool inl = (u.eigen == MB200_EIGEN_INLINE);
             if (u.matrix < 0 || u.matrix >= c.matrix_count || (!inl && !I->std && (u.eigen < 0 || u.eigen >= c.eigen_count)))
-                { rcv = MB200_ERROR_OUT_OF_RANGE; break; }
-            if (inl && (!ev.inline_eigen || S != 4))
-                { rcv = MB200_ERROR_UNSUPPORTED; break; }
+                return MB200_ERROR_OUT_OF_RANGE;
+            if (inl && (!ev.inline_eigen || c.state_count != 4))
+                return MB200_ERROR_UNSUPPORTED;
             if (inl != (ev.matrix_updates[0].eigen == MB200_EIGEN_INLINE))
-                { rcv = MB200_ERROR_UNSUPPORTED; break; }       // all or none of an evaluation's updates
-            I->dirtyOf[u.matrix] = i;
+                return MB200_ERROR_UNSUPPORTED;         // all or none of an evaluation's updates
             }
-        // chunking
-        DevChunk cur = { nOp, 0, (int) cmats.size (), 0 };
-        int curTips = 0;
-        std::vector<int> &touched = I->touched;
-        touched.clear ();
-        auto closeChunk = [&] ()
-            {
-            for (int m : touched) I->slotOf[m] = -1;
-            touched.clear ();
-            DevChunk done = cur;
-            done.nMat |= curTips << 16;
-            chunks.push_back (done);
-            nChunkOf[e]++;
-            cur.opOff += cur.nOp; cur.nOp = 0; cur.matOff = (int) cmats.size (); cur.nMat = 0; curTips = 0;
-            };
-        auto slotFor = [&] (int m) -> int
-            {
-            if (I->slotOf[m] < 0)
-                {
-                I->slotOf[m] = cur.nMat++;
-                touched.push_back (m);
-                DevMat dm; dm.matrix = m;
-                int di = I->dirtyOf[m];
-                if (di <= -2) di = -2 - di;       // already rebuilt in an earlier chunk: rebuild again (other
-                                                  // tiles must not wait for tile 0's copy in the matrix buffer)
-                if (fused && di >= 0) { dm.eigen = ev.matrix_updates[di].eigen; dm.length = ev.matrix_updates[di].length; I->dirtyOf[m] = -2 - di; }
-                else                  { dm.eigen = -1; dm.length = 0.0; }
-                cmats.push_back (dm);
-                }
-            return I->slotOf[m];
-            };
-        for (int i = 0; i < ev.operation_count && rcv == MB200_SUCCESS; i++)
+        for (int i = 0; i < ev.operation_count; i++)
             {
             const mb200_operation &op = ev.operations[i];
             if (!okPartials (I, op.dest, false) || !okPartials (I, op.child1, true) || !okPartials (I, op.child2, true) ||
                 op.matrix1 < 0 || op.matrix1 >= c.matrix_count || op.matrix2 < 0 || op.matrix2 >= c.matrix_count ||
                 (op.child3 != MB200_NONE && (!okPartials (I, op.child3, true) || op.matrix3 < 0 || op.matrix3 >= c.matrix_count)) ||
                 op.scale_write < -1 || op.scale_write >= c.scaler_count || op.scale_remove < -1 || op.scale_remove >= c.scaler_count)
-                { rcv = MB200_ERROR_OUT_OF_RANGE; break; }
-            if (!nuc4)
-                { slots.push_back (-1); slots.push_back (-1); slots.push_back (-1); continue; }
-            const int m3 = (op.child3 == MB200_NONE) ? -1 : op.matrix3;
-            int need = 0;
-            if (I->slotOf[op.matrix1] < 0) need++;
-            if (I->slotOf[op.matrix2] < 0 && op.matrix2 != op.matrix1) need++;
-            if (m3 >= 0 && I->slotOf[m3] < 0 && m3 != op.matrix1 && m3 != op.matrix2) need++;
-            const int tipsHere = (op.child1 < c.tip_count) + (op.child2 < c.tip_count) + (m3 >= 0 && op.child3 < c.tip_count);
-            if (cur.nOp >= opc || cur.nMat + need > maxSlots || curTips + tipsHere > maxTips)
-                closeChunk ();
-            slots.push_back (slotFor (op.matrix1));
-            slots.push_back (slotFor (op.matrix2));
-            slots.push_back (m3 >= 0 ? slotFor (m3) : -1);
-            tipIdx.push_back (op.child1 < c.tip_count ? curTips++ : -1);
-            tipIdx.push_back (op.child2 < c.tip_count ? curTips++ : -1);
-            tipIdx.push_back ((m3 >= 0 && op.child3 < c.tip_count) ? curTips++ : -1);
-            cur.nOp++;
+                return MB200_ERROR_OUT_OF_RANGE;
             }
-        if (nuc4 && rcv == MB200_SUCCESS)
-            {
-            // fused: dirty branches no node of this evaluation reads still have to be rebuilt
-            if (fused)
-                for (int i = 0; i < ev.matrix_update_count; i++)
-                    if (I->dirtyOf[ev.matrix_updates[i].matrix] == i)
-                        {
-                        if (cur.nMat >= maxSlots) closeChunk ();
-                        slotFor (ev.matrix_updates[i].matrix);
-                        }
-            if (cur.nOp > 0 || cur.nMat > 0 || nChunkOf[e] == 0)
-                closeChunk ();
-            for (int m : touched) I->slotOf[m] = -1;
-            touched.clear ();
-            }
-        for (int i = 0; i < ev.matrix_update_count; i++)
-            if (ev.matrix_updates[i].matrix >= 0 && ev.matrix_updates[i].matrix < c.matrix_count)
-                I->dirtyOf[ev.matrix_updates[i].matrix] = -1;
-        nMat += ev.matrix_update_count;
-        nOp  += ev.operation_count;
         }
-    if (rcv != MB200_SUCCESS)
+    return MB200_SUCCESS;
+}
+
+// 4-state family: cut an evaluation's operation list (starting at opOff of the batch) into chunks whose branches
+// fit the kernel's shared-memory P(t) slots, whose nodes fit its node list and whose tip operands fit its lookup
+// tables.  Appends the chunks to I->chunkTmp, their branches to I->cmatTmp and, per operation, three P(t) slots
+// to I->slotTmp and three tip-table indices (-1: not a tip) to I->tipIdxTmp.  Fused: a branch the evaluation
+// rebuilds carries its eigensystem and length, and dirty branches no node reads get slots too.  Returns the
+// number of chunks, at least one.
+int nuc4Chunks (Instance *I, const mb200_evaluation &ev, int opOff, bool fused)
+{
+    const mb200_instance_config &c = I->cfg;
+    const int K = c.category_count;
+    const int maxSlots = nuc_maxs (K), maxTips = nuc_maxt (K), opc = nuc_opc (nuc4PatternsPerBlock (K));   // as in the kernel
+    std::vector<DevChunk> &chunks = I->chunkTmp;
+    std::vector<DevMat>   &cmats = I->cmatTmp;
+    std::vector<int>      &touched = I->touched;        // matrices whose slotOf entry is set (the open chunk's branches)
+    if ((int) I->slotOf.size () < c.matrix_count)
+        { I->slotOf.assign (c.matrix_count, -1); I->dirtyOf.assign (c.matrix_count, -1); }
+    for (int i = 0; i < ev.matrix_update_count; i++)
+        I->dirtyOf[ev.matrix_updates[i].matrix] = i;
+    DevChunk cur = { opOff, 0, (int) cmats.size (), 0 };
+    int curTips = 0, n = 0;
+    auto closeChunk = [&] ()
         {
-        for (int m : I->touched) I->slotOf[m] = -1;
-        I->touched.clear ();
-        return rcv;
+        for (int m : touched) I->slotOf[m] = -1;
+        touched.clear ();
+        DevChunk done = cur;
+        done.nMat |= curTips << 16;
+        chunks.push_back (done);
+        n++;
+        cur.opOff += cur.nOp; cur.nOp = 0; cur.matOff = (int) cmats.size (); cur.nMat = 0; curTips = 0;
+        };
+    auto slotFor = [&] (int m) -> int
+        {
+        if (I->slotOf[m] < 0)
+            {
+            I->slotOf[m] = cur.nMat++;
+            touched.push_back (m);
+            DevMat dm; dm.matrix = m;
+            int di = I->dirtyOf[m];
+            if (di <= -2) di = -2 - di;       // already rebuilt in an earlier chunk: rebuild again (other
+                                              // tiles must not wait for tile 0's copy in the matrix buffer)
+            if (fused && di >= 0) { dm.eigen = ev.matrix_updates[di].eigen; dm.length = ev.matrix_updates[di].length; I->dirtyOf[m] = -2 - di; }
+            else                  { dm.eigen = -1; dm.length = 0.0; }
+            cmats.push_back (dm);
+            }
+        return I->slotOf[m];
+        };
+    for (int i = 0; i < ev.operation_count; i++)
+        {
+        const mb200_operation &op = ev.operations[i];
+        const int m3 = (op.child3 == MB200_NONE) ? -1 : op.matrix3;
+        int need = 0;
+        if (I->slotOf[op.matrix1] < 0) need++;
+        if (I->slotOf[op.matrix2] < 0 && op.matrix2 != op.matrix1) need++;
+        if (m3 >= 0 && I->slotOf[m3] < 0 && m3 != op.matrix1 && m3 != op.matrix2) need++;
+        const int tipsHere = (op.child1 < c.tip_count) + (op.child2 < c.tip_count) + (m3 >= 0 && op.child3 < c.tip_count);
+        if (cur.nOp >= opc || cur.nMat + need > maxSlots || curTips + tipsHere > maxTips)
+            closeChunk ();
+        I->slotTmp.push_back (slotFor (op.matrix1));
+        I->slotTmp.push_back (slotFor (op.matrix2));
+        I->slotTmp.push_back (m3 >= 0 ? slotFor (m3) : -1);
+        I->tipIdxTmp.push_back (op.child1 < c.tip_count ? curTips++ : -1);
+        I->tipIdxTmp.push_back (op.child2 < c.tip_count ? curTips++ : -1);
+        I->tipIdxTmp.push_back ((m3 >= 0 && op.child3 < c.tip_count) ? curTips++ : -1);
+        cur.nOp++;
+        }
+    // fused: dirty branches no node of this evaluation reads still have to be rebuilt
+    if (fused)
+        for (int i = 0; i < ev.matrix_update_count; i++)
+            if (I->dirtyOf[ev.matrix_updates[i].matrix] == i)
+                {
+                if (cur.nMat >= maxSlots) closeChunk ();
+                slotFor (ev.matrix_updates[i].matrix);
+                }
+    if (cur.nOp > 0 || cur.nMat > 0 || n == 0)
+        closeChunk ();
+    for (int i = 0; i < ev.matrix_update_count; i++)
+        I->dirtyOf[ev.matrix_updates[i].matrix] = -1;
+    return n;
+}
+
+// 4-state family: the NucOp records of one evaluation, address-like quantities precomputed and operand kinds
+// resolved.  slots / tipIdx: three per operation, from nuc4Chunks.  Also marks, per chunk, how many operands
+// the latency path fetches when the chunk starts (DevChunk::nMat bits 24+), and where the root comes from.
+void nuc4Encode (Instance *I, const mb200_evaluation &ev, DevEval &d, DevChunk *dc, NucOp *ops,
+                 const int *slots, const int *tipIdx, bool fused)
+{
+    const mb200_instance_config &c = I->cfg;
+    const unsigned bufStride = (unsigned) c.category_count * (unsigned) c.pattern_count;   // float4 per buffer
+    const unsigned slotBytes = (unsigned) c.category_count * 80u;                           // sP[slot][K][5] float4
+    const bool shortcuts = (ev.flags & MB200_FLAG_TIP_SHORTCUTS) != 0;
+    auto chunk = [&] (int q) -> DevChunk & { return q == 0 ? d.chunk0 : dc[d.chunkOff + q - 1]; };
+    std::vector<int> &written = I->writtenTmp;          // [buffer] == stamp: produced earlier in this evaluation
+    if ((int) written.size () < c.partials_count) written.assign (c.partials_count, 0);
+    const int stamp = ++I->writtenStamp;
+    int prevDest = -2, q = 0, opsLeft = d.chunk0.nOp, nPre = 0;
+    auto operand = [&] (int child, unsigned &a) -> unsigned
+        {
+        if (child == MB200_NONE) { a = 0; return NUC_NONE; }
+        if (child < c.tip_count)
+            {
+            a = (unsigned) child * (unsigned) c.pattern_count;
+            return (shortcuts && !I->tipPartAmbig[child]) ? NUC_TIP_ONE : NUC_TIP;
+            }
+        a = (unsigned)(child - c.tip_count) * bufStride;
+        return (child == prevDest) ? NUC_FWD : NUC_LOAD;
+        };
+    for (int i = 0; i < ev.operation_count; i++)
+        {
+        const mb200_operation &op = ev.operations[i];
+        NucOp &o = ops[i];
+        unsigned kind[3] = { operand (op.child1, o.a1), operand (op.child2, o.a2), operand (op.child3, o.a3) };
+        const int child[3] = { op.child1, op.child2, op.child3 };
+        while (opsLeft == 0 && q + 1 < d.nChunk)
+            {
+            chunk (q++).nMat |= nPre << 24;
+            opsLeft = chunk (q).nOp; nPre = 0;
+            }
+        // latency path: interior operands read from buffers this evaluation does not write are
+        // fetched into shared memory when the chunk starts, off the node-to-node chain
+        o.pad = 0;
+        for (int j = 0; j < 3; j++)
+            if (fused && kind[j] == NUC_LOAD && written[child[j]] != stamp && nPre < NUC_MAXPRE)
+                {
+                kind[j] = NUC_PRE;
+                o.pad |= nPre << (4 * j);
+                nPre++;
+                }
+        o.kinds = kind[0] | (kind[1] << 4) | (kind[2] << 8) | (op.scale_write >= 0 ? NUC_RESCALE : 0u);
+        for (int j = 0; j < 3; j++)
+            if (tipIdx[3*i + j] >= 0)
+                o.kinds |= (unsigned) tipIdx[3*i + j] << (13 + 6 * j);
+        o.destOff = (unsigned)(op.dest - c.tip_count) * bufStride;
+        o.sp1 = (unsigned) slots[3*i] * slotBytes;
+        o.sp2 = (unsigned) slots[3*i + 1] * slotBytes;
+        o.sp3 = (slots[3*i + 2] >= 0) ? (unsigned) slots[3*i + 2] * slotBytes : 0u;
+        o.sw = op.scale_write; o.sr = op.scale_remove; o.dest = op.dest;
+        opsLeft--;
+        prevDest = op.dest;
+        written[op.dest] = stamp;
+        }
+    chunk (q).nMat |= nPre << 24;
+    d.rootFwd = (ev.root_buffer != MB200_NONE && ev.root_buffer == prevDest) ? 1 : 0;
+    d.rootOff = (ev.root_buffer != MB200_NONE) ? (unsigned)(ev.root_buffer - c.tip_count) * bufStride : 0u;
+}
+
+// tensor-core path: the nodes of an evaluation are work items of a device-side queue; an item waits for the
+// items that produce its operands.  s1/s2/s3 = producing operation (index within the evaluation) or -1 (tip, or
+// a buffer this evaluation does not write); the queue hands the nodes out level by level (height above the clean
+// operands) so that dependent items sit far apart in it
+void tcOrder (Instance *I, DevOp *ops, int nOp, int *order)
+{
+    const int tips = I->cfg.tip_count;
+    std::vector<int> &producer = I->writtenTmp;         // [buffer] -> operation index + 1 (0: none), reset per evaluation
+    if ((int) producer.size () < I->cfg.partials_count) producer.assign (I->cfg.partials_count, 0);
+    std::vector<int> level (nOp, 0);
+    for (int i = 0; i < nOp; i++)
+        {
+        DevOp &o = ops[i];
+        const int ch[3] = { o.c1, o.c2, o.c3 };
+        int pr[3], lv = 0;
+        for (int j = 0; j < 3; j++)
+            {
+            pr[j] = (ch[j] >= tips && producer[ch[j]] > 0) ? producer[ch[j]] - 1 : -1;
+            if (pr[j] >= 0 && level[pr[j]] + 1 > lv) lv = level[pr[j]] + 1;
+            }
+        o.s1 = pr[0]; o.s2 = pr[1]; o.s3 = pr[2];
+        level[i] = lv;
+        producer[o.dest] = i + 1;
+        }
+    for (int i = 0; i < nOp; i++)
+        producer[ops[i].dest] = 0;
+    int pos = 0;
+    for (int lv = 0; pos < nOp; lv++)
+        for (int i = 0; i < nOp; i++)
+            if (level[i] == lv)
+                order[pos++] = i;
+}
+
+// validate + flatten host evaluations into the device job format
+int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
+{
+    int rc = validate (I, evs, count);
+    if (rc != MB200_SUCCESS)
+        return rc;
+    const mb200_instance_config &c = I->cfg;
+    const int K = c.category_count, S = c.state_count;
+    const bool nuc4 = (S == 4 && K <= 8 && !I->std);
+    // state frequencies per evaluation: S, or the whole table for variable-state divisions (one vector per state count)
+    const int  nFreq = I->std ? MB200_MAX_STATES : S;
+    const long tiles = (c.pattern_count + nuc4PatternsPerBlock (K) - 1) / nuc4PatternsPerBlock (K);
+    // fused P(t) rebuild (every CTA rebuilds the dirty matrices of its evaluation): small launches (latency-
+    // bound regime), and launches of many evaluations over few pattern tiles each (the rebuild is repeated
+    // only tiles-per-evaluation times, and a second kernel + its launch gap would cost more)
+    const bool fused = nuc4 && (tiles * count <= 4L * I->numSMs || tiles <= 16);
+
+    std::vector<DevChunk> &chunks = I->chunkTmp;        // every evaluation's chunks, its first included
+    std::vector<int>      &nChunkOf = I->nChunkTmp;
+    chunks.clear (); I->cmatTmp.clear (); I->slotTmp.clear (); I->tipIdxTmp.clear (); nChunkOf.assign (count, 0);
+    int nMat = 0, nOp = 0;
+    for (int e = 0; e < count; e++)
+        {
+        if (nuc4)
+            nChunkOf[e] = nuc4Chunks (I, evs[e], nOp, fused);
+        nMat += evs[e].matrix_update_count;
+        nOp  += evs[e].operation_count;
         }
 
-    // ---- pass 2: lay the blob out ----
+    // ---- layout ----
     const int nUpd = fused ? 0 : nMat;                 // update list only feeds the stand-alone P(t) kernel
-    int nExtraChunks = 0;
-    for (int e = 0; e < count; e++) nExtraChunks += (nChunkOf[e] > 1) ? nChunkOf[e] - 1 : 0;
+    const int nExtraChunks = (int) chunks.size () - (nuc4 ? count : 0);    // the first chunk lives in the DevEval
     // per evaluation: rates[K], catW[K], freqs[S] and, when the evaluation carries its own
     // eigensystem, the cijk block [2S + S^3]
     int nDbl = 0;
@@ -381,10 +515,10 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
     size_t offUpd   = mb200_align16 (offDbl + sizeof(double) * (size_t)nDbl);
     size_t offChunk = mb200_align16 (offUpd + sizeof(DevMat) * (size_t)nUpd);
     size_t offCmat  = mb200_align16 (offChunk + sizeof(DevChunk) * (size_t)nExtraChunks);
-    size_t offOp    = mb200_align16 (offCmat + sizeof(DevMat) * cmats.size ());
+    size_t offOp    = mb200_align16 (offCmat + sizeof(DevMat) * I->cmatTmp.size ());
     size_t offOrd   = mb200_align16 (offOp + sizeof(DevOp) * (size_t)nOp);      // tensor-core path: level order of the operations
     size_t bytes    = mb200_align16 (offOrd + (I->tcS ? sizeof(int) * (size_t)nOp : 0));
-    int rc = reserveBatch (b, bytes, count);
+    rc = reserveBatch (b, bytes, count);
     if (rc != MB200_SUCCESS)
         return rc;
     DevBatchHeader *h = (DevBatchHeader *) b.hBlob;
@@ -393,17 +527,16 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
     double   *dd = (double   *)(b.hBlob + offDbl);
     DevMat   *du = (DevMat   *)(b.hBlob + offUpd);
     DevChunk *dc = (DevChunk *)(b.hBlob + offChunk);
-    DevMat   *dm = (DevMat   *)(b.hBlob + offCmat);
     DevOp    *dops = (DevOp  *)(b.hBlob + offOp);
     int      *dord = (int    *)(b.hBlob + offOrd);
-    b.maxOps = 0;
-    if (!cmats.empty ())
-        memcpy (dm, cmats.data (), sizeof(DevMat) * cmats.size ());
+    if (!I->cmatTmp.empty ())
+        memcpy (b.hBlob + offCmat, I->cmatTmp.data (), sizeof(DevMat) * I->cmatTmp.size ());
 
-    int mOff = 0, oOff = 0, chunkPos = 0, extraPos = 0, dblPos = 0;
-    b.jx.n = (nuc4 && fused && count <= MB200_JOB_INDEX_MAX) ? count : 0;
-    size_t slotPos = 0;
+    // ---- per evaluation: header, doubles, updates, then the records of its kernel family ----
+    b.maxOps = 0;
     b.needInv = false;
+    b.jx.n = (fused && count <= MB200_JOB_INDEX_MAX) ? count : 0;
+    int mOff = 0, oOff = 0, chunkPos = 0, extraPos = 0, dblPos = 0;
     for (int e = 0; e < count; e++)
         {
         const mb200_evaluation &ev = evs[e];
@@ -428,12 +561,6 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
                 dc[extraPos++] = chunks[chunkPos + q];
             chunkPos += nChunkOf[e];
             }
-        if (nuc4 && fused && count <= MB200_JOB_INDEX_MAX && nChunkOf[e] > 0)
-            {
-            JobIndexEntry &je = b.jx.e[e];
-            je.matOff = d.chunk0.matOff; je.nMat = d.chunk0.nMat; je.opOff = d.chunk0.opOff; je.nOp = d.chunk0.nOp;
-            je.dOff = d.dOff; je.eigen0 = 0;      // eigen0: set below, once known
-            }
         if (d.root != MB200_NONE && d.hasPInvar) b.needInv = true;
         double *dv = dd + d.dOff;
         bool eq = true;
@@ -447,13 +574,7 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
         for (int s = 0; s < nFreq; s++)
             dv[2*K + s] = ev.state_freqs[s];
         if (ev.inline_eigen)
-            {
             memcpy (dv + 2*K + S, ev.inline_eigen, sizeof(double) * (size_t)(2*S + S*S*S));
-            if (ev.matrix_update_count > 0 && ev.matrix_updates[0].eigen == MB200_EIGEN_INLINE)
-                d.eigen0 = MB200_EIGEN_INLINE;
-            }
-        if (e < MB200_JOB_INDEX_MAX)
-            b.jx.e[e].eigen0 = d.eigen0;
         if (!fused)
             for (int i = 0; i < ev.matrix_update_count; i++)
                 {
@@ -463,73 +584,10 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
                 }
         if (nuc4)
             {
-            // 4-state kernels: address-like quantities precomputed, operand kinds resolved
-            const unsigned bufStride = (unsigned) K * (unsigned) c.pattern_count;       // float4 per buffer
-            const unsigned slotBytes = (unsigned) K * 80u;                              // sP[slot][K][5] float4
-            const bool shortcuts = (ev.flags & MB200_FLAG_TIP_SHORTCUTS) != 0;
-            int prevDest = -2;
-            int chunkIdx = chunkPos - nChunkOf[e], opsLeft = (nChunkOf[e] > 0) ? chunks[chunkIdx].nOp : 0, nPre = 0;
-            std::vector<int> &written = I->writtenTmp;      // [buffer] == stamp: produced earlier in this evaluation
-            if ((int) written.size () < c.partials_count) written.assign (c.partials_count, 0);
-            const int stamp = ++I->writtenStamp;
-            auto isWritten = [&] (int buf) { return written[buf] == stamp; };
-            auto operand = [&] (int child, unsigned &a) -> unsigned
-                {
-                if (child == MB200_NONE) { a = 0; return NUC_NONE; }
-                if (child < c.tip_count)
-                    {
-                    a = (unsigned) child * (unsigned) c.pattern_count;
-                    return (shortcuts && !I->tipPartAmbig[child]) ? NUC_TIP_ONE : NUC_TIP;
-                    }
-                a = (unsigned)(child - c.tip_count) * bufStride;
-                return (child == prevDest) ? NUC_FWD : NUC_LOAD;
-                };
-            for (int i = 0; i < ev.operation_count; i++)
-                {
-                const mb200_operation &op = ev.operations[i];
-                NucOp &o = reinterpret_cast<NucOp *>(dops)[oOff + i];
-                const unsigned k1 = operand (op.child1, o.a1), k2 = operand (op.child2, o.a2), k3 = operand (op.child3, o.a3);
-                o.kinds = k1 | (k2 << 4) | (k3 << 8) | (op.scale_write >= 0 ? NUC_RESCALE : 0u);
-                for (int j = 0; j < 3; j++)
-                    if (tipIdx[slotPos + j] >= 0)
-                        o.kinds |= (unsigned) tipIdx[slotPos + j] << (13 + 6 * j);
-                o.destOff = (unsigned)(op.dest - c.tip_count) * bufStride;
-                o.sp1 = (unsigned) slots[slotPos] * slotBytes;
-                o.sp2 = (unsigned) slots[slotPos + 1] * slotBytes;
-                o.sp3 = (slots[slotPos + 2] >= 0) ? (unsigned) slots[slotPos + 2] * slotBytes : 0u;
-                o.sw = op.scale_write; o.sr = op.scale_remove; o.dest = op.dest;
-                // latency path: interior operands read from buffers this evaluation does not write are
-                // fetched into shared memory when the chunk starts, off the node-to-node chain
-                while (opsLeft == 0 && chunkIdx + 1 < chunkPos)
-                    {
-                    (chunkIdx == chunkPos - nChunkOf[e] ? d.chunk0.nMat : dc[d.chunkOff + chunkIdx - (chunkPos - nChunkOf[e]) - 1].nMat) |= nPre << 24;
-                    chunkIdx++; opsLeft = chunks[chunkIdx].nOp; nPre = 0;
-                    }
-                o.pad = 0;
-                if (fused)
-                    {
-                    unsigned kj[3] = { k1, k2, k3 };
-                    const int cj[3] = { op.child1, op.child2, op.child3 };
-                    for (int j = 0; j < 3; j++)
-                        if (kj[j] == NUC_LOAD && !isWritten (cj[j]) && nPre < NUC_MAXPRE)
-                            {
-                            kj[j] = NUC_PRE;
-                            o.pad |= nPre << (4 * j);
-                            nPre++;
-                            }
-                    o.kinds = (o.kinds & ~0xfffu) | kj[0] | (kj[1] << 4) | (kj[2] << 8);
-                    }
-                opsLeft--;
-                slotPos += 3;
-                prevDest = op.dest;
-                written[op.dest] = stamp;
-                }
-            if (nChunkOf[e] > 0)
-                (chunkIdx == chunkPos - nChunkOf[e] ? d.chunk0.nMat : dc[d.chunkOff + chunkIdx - (chunkPos - nChunkOf[e]) - 1].nMat) |= nPre << 24;
-            if (e < MB200_JOB_INDEX_MAX && b.jx.n > 0)
-                b.jx.e[e].nMat = d.chunk0.nMat;
-            d.rootFwd = (ev.root_buffer != MB200_NONE && ev.root_buffer == prevDest) ? 1 : 0;
-            d.rootOff = (ev.root_buffer != MB200_NONE) ? (unsigned)(ev.root_buffer - c.tip_count) * bufStride : 0u;
+            nuc4Encode (I, ev, d, dc, reinterpret_cast<NucOp *>(dops) + oOff, I->slotTmp.data () + 3 * (size_t)oOff,
+                        I->tipIdxTmp.data () + 3 * (size_t)oOff, fused);
+            if (e < b.jx.n)
+                b.jx.e[e] = { d.chunk0.matOff, d.chunk0.nMat, d.chunk0.opOff, d.chunk0.nOp, d.dOff, d.eigen0 };
             }
         else
             {
@@ -540,39 +598,11 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
                 o.dest = op.dest; o.c1 = op.child1; o.m1 = op.matrix1; o.c2 = op.child2; o.m2 = op.matrix2;
                 o.c3 = op.child3; o.m3 = (op.child3 == MB200_NONE) ? MB200_NONE : op.matrix3;
                 o.sw = op.scale_write; o.sr = op.scale_remove;
-                o.s1 = slots[slotPos]; o.s2 = slots[slotPos + 1]; o.s3 = slots[slotPos + 2];
-                slotPos += 3;
+                o.s1 = o.s2 = o.s3 = -1;
                 }
             if (I->tcS)
                 {
-                // tensor-core path: the nodes of an evaluation are work items of a device-side queue; an item waits for
-                // the items that produce its operands.  s1/s2/s3 = producing operation (index within the evaluation)
-                // or -1 (tip, or a buffer this evaluation does not write); the queue hands the nodes out level by
-                // level (height above the clean operands) so that dependent items sit far apart in it
-                std::vector<int> &producer = I->writtenTmp;      // [buffer] -> operation index + 1 (0: none), stamped per evaluation
-                if ((int) producer.size () < c.partials_count) producer.assign (c.partials_count, 0);
-                std::vector<int> level (ev.operation_count, 0);
-                for (int i = 0; i < ev.operation_count; i++)
-                    {
-                    DevOp &o = dops[oOff + i];
-                    const int ch[3] = { o.c1, o.c2, o.c3 };
-                    int pr[3], lv = 0;
-                    for (int j = 0; j < 3; j++)
-                        {
-                        pr[j] = (ch[j] >= c.tip_count && producer[ch[j]] > 0) ? producer[ch[j]] - 1 : -1;
-                        if (pr[j] >= 0 && level[pr[j]] + 1 > lv) lv = level[pr[j]] + 1;
-                        }
-                    o.s1 = pr[0]; o.s2 = pr[1]; o.s3 = pr[2];
-                    level[i] = lv;
-                    producer[o.dest] = i + 1;
-                    }
-                for (int i = 0; i < ev.operation_count; i++)
-                    producer[dops[oOff + i].dest] = 0;
-                int pos = 0;
-                for (int lv = 0; pos < ev.operation_count; lv++)
-                    for (int i = 0; i < ev.operation_count; i++)
-                        if (level[i] == lv)
-                            dord[oOff + pos++] = i;
+                tcOrder (I, dops + oOff, ev.operation_count, dord + oOff);
                 if (ev.operation_count > b.maxOps) b.maxOps = ev.operation_count;
                 }
             }
@@ -601,74 +631,12 @@ int ensureInvMask (Instance *I)
     int C = I->cfg.pattern_count;
     invmask_kernel<<<(C + 255) / 256, 256, 0, I->stream>>> (I->dInvMask, I->dTip64, I->cfg.tip_count, C);
     CK (cudaGetLastError ());
-    I->launches++; I->launchKind[MB200_KERNEL_SETUP]++;
+    I->launchKind[MB200_KERNEL_SETUP]++;
     I->invMaskValid = true;
     return MB200_SUCCESS;
 }
 
-// launch one instantiation of the 4-state kernel; the first launch per device opts it in to its
-// dynamic shared-memory size
-template <int KK, int NT, bool F>
-int launchNuc4K (Instance *I, const DevCtx &ctx, dim3 grid, const DevEval *de, const double *dd, const DevChunk *dc,
-                 const DevMat *dm, const DevOp *dops, DevResult *res, int seq, const JobIndex &jx)
-{
-    static bool optedIn[64];
-    auto kern = eval_nuc4_kernel<KK, NT, F>;
-    constexpr int bytes = (int) sizeof(Nuc4Smem<KK, NT, F>);
-    if (!optedIn[I->cfg.device & 63])
-        {
-        CK (cudaFuncSetAttribute (kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-        optedIn[I->cfg.device & 63] = true;
-        }
-    kern<<<grid, NT, bytes, I->stream>>> (ctx, de, dd, dc, dm, dops, res, seq, jx);
-    return MB200_SUCCESS;
-}
-
-template <int KK, int NT, int CAP>
-int launchNuc4PK (Instance *I, const DevCtx &ctx, dim3 grid, const ParamBlob<CAP> &blob, const BlobOffsets &off, DevResult *res, int seq,
-                  const JobIndex &jx)
-{
-    static bool optedIn[64];
-    auto kern = eval_nuc4_pkernel<KK, NT, CAP>;
-    constexpr int bytes = (int) sizeof(Nuc4Smem<KK, NT, true>);
-    if (!optedIn[I->cfg.device & 63])
-        {
-        CK (cudaFuncSetAttribute (kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-        optedIn[I->cfg.device & 63] = true;
-        }
-    kern<<<grid, NT, bytes, I->stream>>> (ctx, off, res, seq, jx, blob);
-    return MB200_SUCCESS;
-}
-
-int launchNuc4 (Instance *I, const DevCtx &ctx, dim3 grid, const DevEval *de, const double *dd, const DevChunk *dc,
-                const DevMat *dm, const DevOp *dops, DevResult *res, int seq, bool fused, const JobIndex &jx)
-{
-    switch (ctx.K)
-        {
-#define MB200_CASE(KK) case KK: return fused ? launchNuc4K<KK, NT_NUC4, true> (I, ctx, grid, de, dd, dc, dm, dops, res, seq, jx) \
-                                              : launchNuc4K<KK, NT_NUC4, false> (I, ctx, grid, de, dd, dc, dm, dops, res, seq, jx);
-        MB200_CASE(1) MB200_CASE(2) MB200_CASE(3) MB200_CASE(4) MB200_CASE(5) MB200_CASE(6) MB200_CASE(7) MB200_CASE(8)
-#undef MB200_CASE
-        default: return MB200_ERROR_UNSUPPORTED;
-        }
-}
-
-// the same kernel with the job descriptors riding in the parameter block (no H2D copy)
-template <int CAP>
-int launchNuc4Param (Instance *I, const DevCtx &ctx, dim3 grid, const Batch &b, DevResult *res, int seq)
-{
-    const ParamBlob<CAP> &blob = *reinterpret_cast<const ParamBlob<CAP> *>(b.hBlob);
-    BlobOffsets off = { (int) b.offEval, (int) b.offDbl, (int) b.offUpd, (int) b.offChunk, (int) b.offCmat, (int) b.offOp };
-    switch (ctx.K)
-        {
-#define MB200_CASE(KK) case KK: return launchNuc4PK<KK, NT_NUC4, CAP> (I, ctx, grid, blob, off, res, seq, b.jx);
-        MB200_CASE(1) MB200_CASE(2) MB200_CASE(3) MB200_CASE(4) MB200_CASE(5) MB200_CASE(6) MB200_CASE(7) MB200_CASE(8)
-#undef MB200_CASE
-        default: return MB200_ERROR_UNSUPPORTED;
-        }
-}
-
-const int PARAM_SMALL = 4096, PARAM_MID = 10240, PARAM_BIG = 30720;   // parameter-block sizes compiled (the launch copies all of it)
+constexpr int PARAM_SMALL = 4096, PARAM_MID = 10240, PARAM_BIG = 30720;   // parameter-block sizes compiled (the launch copies all of it)
 
 bool paramEligible (const Instance *I, const Batch &b)
 {
@@ -677,9 +645,63 @@ bool paramEligible (const Instance *I, const Batch &b)
 
 const int TC_MIN_ROWS = 128;    // rows (site patterns) per tile of the tensor-core kernel = the MMA's M
 
-// launch the fused pass for a packed batch; fromHost: the job lives in b.hBlob only and is
-// delivered through the parameter block when it fits (otherwise the caller has copied it to dBlob)
-int launch (Instance *I, Batch &b, DevResult *res, bool viaParams, bool hostSum = false)
+// 4-state instance (at creation): opt the five launched 4-state kernels of its K in to their dynamic shared
+// memory.  The resident kernel may serve the instance if its whole grid (tiles x maxEval) fits the device at
+// once -- every CTA must be running for a job to complete; if it cannot be opted in or its occupancy cannot
+// be queried, the instance keeps its launches
+int nuc4Setup (Instance *I)
+{
+    return withNuc4K (I->cfg.category_count, [&] (auto k)
+        {
+        constexpr int KK = decltype (k)::value;
+        const cudaFuncAttribute dyn = cudaFuncAttributeMaxDynamicSharedMemorySize;
+        CK (cudaFuncSetAttribute (eval_nuc4_kernel<KK, NT_NUC4, true>, dyn, nuc4Smem<KK, true>));
+        CK (cudaFuncSetAttribute (eval_nuc4_kernel<KK, NT_NUC4, false>, dyn, nuc4Smem<KK, false>));
+        CK (cudaFuncSetAttribute (eval_nuc4_pkernel<KK, NT_NUC4, PARAM_SMALL>, dyn, nuc4Smem<KK, true>));
+        CK (cudaFuncSetAttribute (eval_nuc4_pkernel<KK, NT_NUC4, PARAM_MID>, dyn, nuc4Smem<KK, true>));
+        CK (cudaFuncSetAttribute (eval_nuc4_pkernel<KK, NT_NUC4, PARAM_BIG>, dyn, nuc4Smem<KK, true>));
+        int perSM = 0;
+        if (cudaFuncSetAttribute (eval_nuc4_resident_kernel<KK, NT_NUC4>, dyn, nuc4Smem<KK, true>) != cudaSuccess ||
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor (&perSM, eval_nuc4_resident_kernel<KK, NT_NUC4>, NT_NUC4, nuc4Smem<KK, true>) != cudaSuccess)
+            { cudaGetLastError (); perSM = 0; }
+        I->resOk = (long) perSM * I->numSMs >= (long) I->maxTiles * I->maxEval;
+        return MB200_SUCCESS;
+        });
+}
+
+// tensor-core instance of S states (at creation): the pipelined kernel gets as many operand-ring stages as
+// fit next to its static shared memory, and is opted in to the dynamic shared memory they take (tcpStages
+// stays 0 when none fits).  Returns the floats of one pre-split P(t) image.
+template <int S>
+size_t tcSetup (Instance *I)
+{
+    const int K = I->cfg.category_count;
+    int optin = 0;
+    cudaDeviceGetAttribute (&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, I->cfg.device);
+    cudaFuncAttributes fa;
+    const size_t staticBytes = (cudaFuncGetAttributes (&fa, eval_tcp_kernel<S>) == cudaSuccess) ? fa.sharedSizeBytes : 4096;    // barriers, item ring, row maxima
+    const size_t limit = ((size_t) optin > staticBytes + 1024) ? (size_t) optin - staticBytes : 0;
+    I->tcpStages = tcp_stages<S> (K, limit);
+    if (I->tcpStages > 0)
+        {
+        I->tcpSmem = I->tcpStages * tcp_stage_bytes<S> () + tcp_staging_bytes<S> (K) + tcp_tipring_bytes<S> (I->tcpStages);
+        if (cudaFuncSetAttribute (eval_tcp_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) I->tcpSmem) != cudaSuccess)
+            { cudaGetLastError (); I->tcpStages = 0; }
+        }
+    return tc_split_floats<S> ();
+}
+
+// make the evaluation just launched or posted the instance's pending one: runEnd () and retire () read
+// only this record
+void setPending (Instance *I, Batch &b, int seq, bool resident, bool hostSum, int tiles)
+{
+    I->pending = { b.nEval, seq, &b, resident, hostSum, tiles };
+}
+
+// launch the evaluation of a packed batch.  viaParams: the job lives in b.hBlob only and rides in the
+// parameter block (otherwise the caller has copied it to dBlob).  toHost: the results go to the batch's
+// mapped host buffer and the launch becomes the pending evaluation; else they go to b.dRes.
+int launch (Instance *I, Batch &b, bool viaParams, bool toHost)
 {
     const DevEval  *de = (const DevEval  *)(b.dBlob + b.offEval);
     const double   *dd = (const double   *)(b.dBlob + b.offDbl);
@@ -687,6 +709,7 @@ int launch (Instance *I, Batch &b, DevResult *res, bool viaParams, bool hostSum 
     const DevChunk *dc = (const DevChunk *)(b.dBlob + b.offChunk);
     const DevMat   *dm = (const DevMat   *)(b.dBlob + b.offCmat);
     const DevOp    *dops = (const DevOp  *)(b.dBlob + b.offOp);
+    DevResult *res = toHost ? b.hResDev : b.dRes;
     DevCtx ctx = I->ctx;
     const int seq = ++I->seq;
 
@@ -699,7 +722,7 @@ int launch (Instance *I, Batch &b, DevResult *res, bool viaParams, bool hostSum 
         {
         tiprobs_std_kernel<<<b.nMat, 64, 0, I->stream>>> (ctx, I->sx, de, b.nEval, dd, du);
         CK (cudaGetLastError ());
-        I->launches++; I->launchKind[MB200_KERNEL_TIPROBS]++;
+        I->launchKind[MB200_KERNEL_TIPROBS]++;
         }
     else if (b.nDirty > 0 && !b.fused)
         {
@@ -716,7 +739,7 @@ int launch (Instance *I, Batch &b, DevResult *res, bool viaParams, bool hostSum 
             tiprobs_kernel<<<grid, 128, 0, I->stream>>> (ctx, de, b.nEval, dd, du);
             }
         CK (cudaGetLastError ());
-        I->launches++; I->launchKind[MB200_KERNEL_TIPROBS]++;
+        I->launchKind[MB200_KERNEL_TIPROBS]++;
         }
     const int evSlot = (int)(I->evCount % EV_RING);
     if (I->timing)
@@ -745,47 +768,61 @@ int launch (Instance *I, Batch &b, DevResult *res, bool viaParams, bool hostSum 
         // instead of once per tile.  Single-chunk evaluations only (per-pattern state lives in registers).
         if (b.fused && (I->cfg.flags & MB200_CONFIG_THROUGHPUT) && b.singleChunk)
             ctx.numTiles = 1;
-        ctx.hostSum = (hostSum && ctx.numTiles <= HOSTSUM_MAX_TILES) ? 1 : 0;
-        I->lastHostSum = ctx.hostSum; I->lastTiles = ctx.numTiles;
-        dim3 grid (ctx.numTiles, b.nEval);
-        int rc;
-        if (viaParams)
+        ctx.hostSum = (toHost && b.allRoot && b.fused && ctx.numTiles <= HOSTSUM_MAX_TILES) ? 1 : 0;
+        const dim3 grid (ctx.numTiles, b.nEval);
+        const BlobOffsets off = { (int) b.offEval, (int) b.offDbl, (int) b.offUpd, (int) b.offChunk, (int) b.offCmat, (int) b.offOp };
+        int rc = withNuc4K (ctx.K, [&] (auto k)
             {
-            if (b.bytes <= (size_t) PARAM_SMALL)    rc = launchNuc4Param<PARAM_SMALL> (I, ctx, grid, b, res, seq);
-            else if (b.bytes <= (size_t) PARAM_MID) rc = launchNuc4Param<PARAM_MID> (I, ctx, grid, b, res, seq);
-            else                                    rc = launchNuc4Param<PARAM_BIG> (I, ctx, grid, b, res, seq);
-            }
-        else
-            rc = launchNuc4 (I, ctx, grid, de, dd, dc, dm, dops, res, seq, b.fused, b.jx);
+            constexpr int KK = decltype (k)::value;
+            // the job descriptors in the parameter block (no H2D copy); the launch copies all CAP bytes
+            auto viaBlock = [&] (auto cap)
+                {
+                constexpr int CAP = decltype (cap)::value;
+                eval_nuc4_pkernel<KK, NT_NUC4, CAP><<<grid, NT_NUC4, nuc4Smem<KK, true>, I->stream>>> (
+                    ctx, off, res, seq, b.jx, *reinterpret_cast<const ParamBlob<CAP> *>(b.hBlob));
+                };
+            if (!viaParams && b.fused)
+                eval_nuc4_kernel<KK, NT_NUC4, true><<<grid, NT_NUC4, nuc4Smem<KK, true>, I->stream>>> (ctx, de, dd, dc, dm, dops, res, seq, b.jx);
+            else if (!viaParams)
+                eval_nuc4_kernel<KK, NT_NUC4, false><<<grid, NT_NUC4, nuc4Smem<KK, false>, I->stream>>> (ctx, de, dd, dc, dm, dops, res, seq, b.jx);
+            else if (b.bytes <= (size_t) PARAM_SMALL)
+                viaBlock (std::integral_constant<int, PARAM_SMALL> ());
+            else if (b.bytes <= (size_t) PARAM_MID)
+                viaBlock (std::integral_constant<int, PARAM_MID> ());
+            else
+                viaBlock (std::integral_constant<int, PARAM_BIG> ());
+            return MB200_SUCCESS;
+            });
         if (rc != MB200_SUCCESS) return rc;
         I->launchKind[MB200_KERNEL_NUC4]++;
         }
     else if (I->tcS)
         {
-        // tensor-core path: refresh the pre-split images of the matrices just rebuilt, then prune
-        // (61 states: tiprobs_mm_kernel has written them already)
-        if (b.nDirty > 0 && I->tcS != 61)
-            {
-            dim3 sg (b.nMat, ctx.K);
-            tc_split_kernel<20><<<sg, 128, 0, I->stream>>> (I->dMatrices, I->dSplit, du, 0, ctx.K);
-            CK (cudaGetLastError ());
-            I->launches++; I->launchKind[MB200_KERNEL_SETUP]++;
-            }
-        {
-        // warp-specialised pipeline over the node-parallel queue: one persistent CTA per SM
         ctx.tilePatterns = 128;
         ctx.numTiles = (ctx.C + 127) / 128;
-        TcQueue Q;
-        Q.counter = I->dTcCounter; Q.base = I->tcBase; Q.flags = I->dTcFlags; Q.flagStride = I->tcFlagStride;
-        Q.maxOps = b.maxOps; Q.nEval = b.nEval; Q.error = I->dTcError; Q.order = (const int *)(b.dBlob + b.offOrd);
-        const long total = (long)(b.maxOps + 1) * b.nEval * ctx.numTiles;
-        const int  g = (int)((total < (long) I->numSMs) ? total : (long) I->numSMs);
-        I->tcBase += (unsigned int)(total + g);                  // every CTA draws exactly one ticket past the end
-        if (I->tcS == 61)
-            eval_tcp_kernel<61><<<g, TCP_THREADS, I->tcpSmem, I->stream>>> (ctx, Q, I->tcpStages, de, dd, dops, I->dSplit, res, seq);
-        else
-            eval_tcp_kernel<20><<<g, TCP_THREADS, I->tcpSmem, I->stream>>> (ctx, Q, I->tcpStages, de, dd, dops, I->dSplit, res, seq);
-        }
+        int rc = withTcS (I->tcS, [&] (auto s)
+            {
+            constexpr int TS = decltype (s)::value;
+            // refresh the pre-split images of the matrices just rebuilt (61 states: tiprobs_mm_kernel has
+            // written them already)
+            if constexpr (TS != 61)
+                if (b.nDirty > 0)
+                    {
+                    tc_split_kernel<TS><<<dim3 (b.nMat, ctx.K), 128, 0, I->stream>>> (I->dMatrices, I->dSplit, du, 0, ctx.K);
+                    CK (cudaGetLastError ());
+                    I->launchKind[MB200_KERNEL_SETUP]++;
+                    }
+            // warp-specialised pipeline over the node-parallel queue: one persistent CTA per SM
+            TcQueue Q;
+            Q.counter = I->dTcCounter; Q.base = I->tcBase; Q.flags = I->dTcFlags; Q.flagStride = I->tcFlagStride;
+            Q.maxOps = b.maxOps; Q.nEval = b.nEval; Q.error = I->dTcError; Q.order = (const int *)(b.dBlob + b.offOrd);
+            const long total = (long)(b.maxOps + 1) * b.nEval * ctx.numTiles;
+            const int  g = (int)((total < (long) I->numSMs) ? total : (long) I->numSMs);
+            I->tcBase += (unsigned int)(total + g);                  // every CTA draws exactly one ticket past the end
+            eval_tcp_kernel<TS><<<g, TCP_THREADS, I->tcpSmem, I->stream>>> (ctx, Q, I->tcpStages, de, dd, dops, I->dSplit, res, seq);
+            return MB200_SUCCESS;
+            });
+        if (rc != MB200_SUCCESS) return rc;
         I->launchKind[MB200_KERNEL_TENSOR]++;
         }
     else
@@ -794,12 +831,13 @@ int launch (Instance *I, Batch &b, DevResult *res, bool viaParams, bool hostSum 
         I->launchKind[MB200_KERNEL_GENERIC]++;
         }
     CK (cudaGetLastError ());
-    I->launches++;
     if (I->timing)
         {
         CK (cudaEventRecord (I->evB[evSlot], I->stream));
         I->evCount++;
         }
+    if (toHost)
+        setPending (I, b, seq, false, ctx.hostSum != 0, ctx.numTiles);
     return MB200_SUCCESS;
 }
 
@@ -843,37 +881,6 @@ void post (Instance *I, int seq, int count, const Batch *b)
     __atomic_signal_fence (__ATOMIC_SEQ_CST);
 }
 
-// K-dispatch of the resident kernel: with `go` false only checks that the whole grid fits the device
-// at once (every CTA must be running for a job to complete)
-template <int KK>
-int residentKernel (Instance *I, const DevCtx &ctx, dim3 grid, int seq0, bool go)
-{
-    auto kern = eval_nuc4_resident_kernel<KK, NT_NUC4>;
-    constexpr int bytes = (int) sizeof(Nuc4Smem<KK, NT_NUC4, true>);
-    if (!go)
-        {
-        int perSM = 0;
-        CK (cudaFuncSetAttribute (kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-        CK (cudaOccupancyMaxActiveBlocksPerMultiprocessor (&perSM, kern, NT_NUC4, bytes));
-        I->resFits = ((long) perSM * I->numSMs >= (long) grid.x * grid.y) ? 1 : 0;
-        return MB200_SUCCESS;
-        }
-    kern<<<grid, NT_NUC4, bytes, I->stream>>> (ctx, I->hMailDev, I->dJob, seq0, RES_IDLE_NS);
-    CK (cudaGetLastError ());
-    return MB200_SUCCESS;
-}
-
-int residentDispatch (Instance *I, const DevCtx &ctx, dim3 grid, int seq0, bool go)
-{
-    switch (ctx.K)
-        {
-#define MB200_CASE(KK) case KK: return residentKernel<KK> (I, ctx, grid, seq0, go);
-        MB200_CASE(1) MB200_CASE(2) MB200_CASE(3) MB200_CASE(4) MB200_CASE(5) MB200_CASE(6) MB200_CASE(7) MB200_CASE(8)
-#undef MB200_CASE
-        default: return MB200_ERROR_UNSUPPORTED;
-        }
-}
-
 DevCtx residentCtx (const Instance *I)
 {
     DevCtx ctx = I->ctx;
@@ -892,12 +899,10 @@ DevCtx residentCtx (const Instance *I)
 bool residentEligible (Instance *I, const Batch &b)
 {
     const mb200_instance_config &c = I->cfg;
-    if (I->std || c.state_count != 4 || c.category_count > 8 || I->timing ||
-        (c.flags & MB200_CONFIG_THROUGHPUT) || !b.fused || !b.allRoot || b.nEval > MB200_JOB_INDEX_MAX || b.jx.n != b.nEval ||
-        I->maxEval > MB200_JOB_INDEX_MAX || I->resFits == 0)
+    if (!I->resOk || I->timing || (c.flags & MB200_CONFIG_THROUGHPUT) || !b.fused || !b.allRoot ||
+        b.nEval > MB200_JOB_INDEX_MAX || b.jx.n != b.nEval || I->maxEval > MB200_JOB_INDEX_MAX)
         return false;
-    const DevCtx ctx = residentCtx (I);
-    if (ctx.numTiles > HOSTSUM_MAX_TILES)
+    if (residentCtx (I).numTiles > HOSTSUM_MAX_TILES)
         return false;
     {
     std::lock_guard<std::mutex> g (gLock);
@@ -907,21 +912,21 @@ bool residentEligible (Instance *I, const Batch &b)
     if (live != 1)
         return false;
     }
-    if (I->resFits < 0)
+    if (!I->dJob)
         {
+        // mailbox and job copy on first use; without them the instance keeps its launches
         if (cudaHostAlloc ((void **)&I->hMail, sizeof(int4) * MB200_RES_PIECES, cudaHostAllocMapped) != cudaSuccess ||
             cudaHostGetDevicePointer ((void **)&I->hMailDev, I->hMail, 0) != cudaSuccess ||
             cudaMalloc ((void **)&I->dJob, sizeof(ResidentJob)) != cudaSuccess ||
-            cudaMemset (I->dJob, 0, sizeof(ResidentJob)) != cudaSuccess ||
-            residentDispatch (I, ctx, dim3 (ctx.numTiles, I->maxEval), 0, false) != MB200_SUCCESS)
+            cudaMemset (I->dJob, 0, sizeof(ResidentJob)) != cudaSuccess)
             {
             cudaGetLastError ();
-            I->resFits = 0;
+            I->resOk = false;
             return false;
             }
         memset (I->hMail, 0, sizeof(int4) * MB200_RES_PIECES);
         }
-    return I->resFits == 1;
+    return true;
 }
 
 // post batch b, launching a resident kernel first when none is running
@@ -944,29 +949,37 @@ int residentStart (Instance *I, Batch &b)
     post (I, seq, b.nEval, &b);
     if (!I->resident)
         {
-        int rc = residentDispatch (I, ctx, dim3 (ctx.numTiles, I->maxEval), seq0, true);
+        const dim3 grid (ctx.numTiles, I->maxEval);
+        int rc = withNuc4K (ctx.K, [&] (auto k)
+            {
+            constexpr int KK = decltype (k)::value;
+            eval_nuc4_resident_kernel<KK, NT_NUC4><<<grid, NT_NUC4, nuc4Smem<KK, true>, I->stream>>> (ctx, I->hMailDev, I->dJob, seq0, RES_IDLE_NS);
+            CK (cudaGetLastError ());
+            return MB200_SUCCESS;
+            });
         if (rc != MB200_SUCCESS) return rc;
         I->resident = true;
-        I->launches++; I->launchKind[MB200_KERNEL_NUC4]++;
+        I->launchKind[MB200_KERNEL_NUC4]++;
         }
-    I->lastHostSum = 1; I->lastTiles = ctx.numTiles;
-    I->pendingSeq = seq; I->pendingResident = true; I->resBatch = &b;
+    setPending (I, b, seq, true, true, ctx.numTiles);
     return MB200_SUCCESS;
 }
 
-// wait until the kernel has written `slots` results into the mapped host buffer.  While a resident
-// kernel serves the instance the stream never goes idle, so the wait has a wall-clock deadline; an
+// wait until the kernel has written the pending evaluation's results into the mapped host buffer.  While a
+// resident kernel serves the instance the stream never goes idle, so the wait has a wall-clock deadline; an
 // idle stream then means the kernel exited on its timeout before its leader took the post, so no CTA
 // ran the job and it is posted again to a new kernel.
-int waitResults (Instance *I, Batch &b, int slots)
+int waitResults (Instance *I)
 {
-    volatile DevResult *r = b.hRes;
+    const Pending &p = I->pending;             // a relaunch below records the same evaluation with a new seq
+    volatile DevResult *r = p.batch->hRes;
+    const int slots = p.hostSum ? p.count * p.tiles : p.count;
     unsigned long long spins = 0;
     const double t0 = wallNow ();
     for (int e = 0; e < slots; e++)
         {
-        // pendingSeq: the launch or post begin() issued, whatever else ran on the instance since
-        while (r[e].seq != I->pendingSeq)
+        // p.seq: the launch or post begin() issued, whatever else ran on the instance since
+        while (r[e].seq != p.seq)
             {
 #if defined(__x86_64__)
             __builtin_ia32_pause ();
@@ -976,17 +989,17 @@ int waitResults (Instance *I, Batch &b, int slots)
                 cudaError_t q = cudaStreamQuery (I->stream);
                 if (q == cudaSuccess)
                     {
-                    if (r[e].seq == I->pendingSeq) break;
-                    if (I->resident && I->pendingResident)
+                    if (r[e].seq == p.seq) break;
+                    if (I->resident && p.resident)
                         {
                         for (int i = 0; i < slots; i++)
-                            if (r[i].seq == I->pendingSeq)
+                            if (r[i].seq == p.seq)
                                 {
                                 fprintf (stderr, "mb200: resident kernel exited in the middle of a job\n");
                                 return MB200_ERROR_GENERAL;
                                 }
                         I->resident = false;
-                        int rc = residentStart (I, *I->resBatch);
+                        int rc = residentStart (I, *p.batch);
                         if (rc != MB200_SUCCESS) return rc;
                         e = -1;                 // every slot again, for the new sequence number
                         break;
@@ -1018,9 +1031,9 @@ int retire (Instance *I)
 {
     if (!I->resident)
         return MB200_SUCCESS;
-    if (I->pendingCount > 0 && I->pendingResident)
+    if (I->pending.count > 0 && I->pending.resident)
         {
-        int rc = waitResults (I, *I->pendingBatch, I->pendingCount * I->lastTiles);
+        int rc = waitResults (I);
         if (rc != MB200_SUCCESS) return rc;
         }
     I->resident = false;
@@ -1032,7 +1045,7 @@ int retire (Instance *I)
 // first half of an evaluation: validate, pack, launch.  Returns as soon as the work is queued.
 int runBegin (Instance *I, const mb200_evaluation *evs, int count)
 {
-    if (I->pendingCount > 0)
+    if (I->pending.count > 0)
         return MB200_ERROR_OUT_OF_RANGE;               // one evaluation in flight per instance
     Batch &b = I->scratch;
     int rc = pack (I, b, evs, count);
@@ -1040,42 +1053,34 @@ int runBegin (Instance *I, const mb200_evaluation *evs, int count)
     const bool viaParams = paramEligible (I, b);
     if (!viaParams)
         CK (cudaMemcpyAsync (b.dBlob, b.hBlob, b.bytes, cudaMemcpyHostToDevice, I->stream));
-    I->lastHostSum = 0; I->lastTiles = 1;
-    rc = launch (I, b, b.hResDev, viaParams, b.allRoot && b.fused);
-    if (rc != MB200_SUCCESS) return rc;
-    I->pendingCount = count; I->pendingBatch = &b; I->pendingSeq = I->seq; I->pendingResident = false;
-    return MB200_SUCCESS;
+    return launch (I, b, viaParams, true);
 }
 
-// second half: wait for the results of the evaluation started by runBegin
+// second half: wait for the results of the pending evaluation
 int runEnd (Instance *I, double *lnL, int *status)
 {
-    const int count = I->pendingCount;
-    if (count <= 0)
+    if (I->pending.count <= 0)
         return MB200_ERROR_OUT_OF_RANGE;
-    I->pendingCount = 0;
-    Batch &b = *I->pendingBatch;
-    if (b.allRoot)
-        {
-        // results land in pinned host memory; no D2H copy, no stream synchronisation
-        int rc = waitResults (I, b, I->lastHostSum ? count * I->lastTiles : count);
-        I->pendingResident = false;
-        if (rc != MB200_SUCCESS) return rc;
-        }
-    else
+    const Pending p = I->pending;                      // a relaunch inside the wait changes only its seq
+    const Batch &b = *p.batch;
+    // results land in pinned host memory; no D2H copy, no stream synchronisation
+    const int rc = b.allRoot ? waitResults (I) : MB200_SUCCESS;
+    I->pending = Pending ();
+    if (rc != MB200_SUCCESS) return rc;
+    if (!b.allRoot)
         CK (cudaStreamSynchronize (I->stream));
-    for (int e = 0; e < count; e++)
+    for (int e = 0; e < p.count; e++)
         {
         if (b.hasRoot[e])
             {
-            if (I->lastHostSum)
+            if (p.hostSum)
                 {
                 // the tiles' partial sums, added left to right (the order the device uses too)
                 double tot = 0.0; int ab = 0;
-                for (int t = 0; t < I->lastTiles; t++)
+                for (int t = 0; t < p.tiles; t++)
                     {
-                    tot += b.hRes[e * I->lastTiles + t].lnL;
-                    ab  |= b.hRes[e * I->lastTiles + t].status;
+                    tot += b.hRes[e * p.tiles + t].lnL;
+                    ab  |= b.hRes[e * p.tiles + t].status;
                     }
                 if (lnL)    lnL[e] = ab ? -DBL_MAX : tot;
                 if (status) status[e] = ab ? MB200_EVAL_UNDERFLOW : MB200_EVAL_OK;
@@ -1256,10 +1261,12 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
         }
     if (I->tcS)
         {
-        const size_t fl = (I->tcS == 61) ? tc_split_floats<61> () : tc_split_floats<20> ();
+        // warp-specialised pipelined kernel: one CTA per SM, as many operand-ring stages as fit
+        const size_t fl = withTcS (I->tcS, [&] (auto s) { return tcSetup<decltype (s)::value> (I); });
+        if (I->tcpStages == 0)
+            { destroy (I); return MB200_ERROR_UNSUPPORTED; }     // cannot happen for K <= 4 on a 227 KB part
         ALLOC (I->dSplit, (size_t)cfg->matrix_count * K * fl * sizeof(float));
         cudaMemsetAsync (I->dSplit, 0, (size_t)cfg->matrix_count * K * fl * sizeof(float), I->stream);
-        cudaError_t ea;
         I->tcFlagStride = (int) nInt + 1;
         const size_t nFlags = (size_t) I->maxEval * ((size_t)(C + TC_MIN_ROWS - 1) / TC_MIN_ROWS + 1) * I->tcFlagStride;
         ALLOC (I->dTcCounter, sizeof(unsigned int));
@@ -1268,26 +1275,6 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
         cudaMemsetAsync (I->dTcCounter, 0, sizeof(unsigned int), I->stream);
         cudaMemsetAsync (I->dTcError, 0, sizeof(int), I->stream);
         cudaMemsetAsync (I->dTcFlags, 0, nFlags * sizeof(int), I->stream);
-        // warp-specialised pipelined kernel: one CTA per SM, as many operand-ring stages as fit
-        {
-        int optin = 0;
-        cudaDeviceGetAttribute (&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, I->cfg.device);
-        cudaFuncAttributes fa;
-        ea = (I->tcS == 61) ? cudaFuncGetAttributes (&fa, eval_tcp_kernel<61>) : cudaFuncGetAttributes (&fa, eval_tcp_kernel<20>);
-        const size_t staticBytes = (ea == cudaSuccess) ? fa.sharedSizeBytes : 4096;    // barriers, item ring, row maxima
-        const size_t limit = ((size_t) optin > staticBytes + 1024) ? (size_t) optin - staticBytes : 0;
-        I->tcpStages = (I->tcS == 61) ? tcp_stages<61> (K, limit) : tcp_stages<20> (K, limit);
-        if (I->tcpStages > 0)
-            {
-            I->tcpSmem = (I->tcS == 61) ? I->tcpStages * tcp_stage_bytes<61> () + tcp_staging_bytes<61> (K) + tcp_tipring_bytes<61> (I->tcpStages)
-                                        : I->tcpStages * tcp_stage_bytes<20> () + tcp_staging_bytes<20> (K) + tcp_tipring_bytes<20> (I->tcpStages);
-            ea = (I->tcS == 61) ? cudaFuncSetAttribute (eval_tcp_kernel<61>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) I->tcpSmem)
-                                : cudaFuncSetAttribute (eval_tcp_kernel<20>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) I->tcpSmem);
-            if (ea != cudaSuccess) { cudaGetLastError (); I->tcpStages = 0; }
-            }
-        if (I->tcpStages == 0)
-            { destroy (I); return MB200_ERROR_UNSUPPORTED; }     // cannot happen for K <= 4 on a 227 KB part
-        }
         }
     ALLOC (I->dInvMask,  (size_t)C * sizeof(uint64_t));
     ALLOC (I->dTilePartial, (size_t)I->maxEval * I->maxTiles * sizeof(double));
@@ -1319,6 +1306,8 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
         if (cudaFuncSetAttribute (eval_gen_kernel<NT_GEN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) I->smemGen) != cudaSuccess)
             { destroy (I); return MB200_ERROR_CUDA; }
         }
+    if (nuc4 && nuc4Setup (I) != MB200_SUCCESS)
+        { destroy (I); return MB200_ERROR_CUDA; }
 
     DevCtx &x = I->ctx;
     memset (&x, 0, sizeof(x));
@@ -1461,7 +1450,7 @@ int mb200_set_cijk (int instance, int eigen, const double *block)
         cijk_factor_kernel<<<dim3 (S, I->cijkParts), 256, 0, I->stream>>> (I->dEigen + (size_t)eigen * I->eigenStride,
                                                                             I->dFactor + (size_t)eigen * I->cijkParts * 2 * S * S, S);
         CK (cudaGetLastError ());
-        I->launches++; I->launchKind[MB200_KERNEL_SETUP]++;
+        I->launchKind[MB200_KERNEL_SETUP]++;
         }
     CK (cudaStreamSynchronize (I->stream));
     return MB200_SUCCESS;
@@ -1485,7 +1474,7 @@ int mb200_set_eigen_decomposition (int instance, int eigen, const double *V, con
     size_t n3 = n2 * S;
     int blocks = (int)((n3 + 255) / 256); if (blocks > 1024) blocks = 1024;
     cijk_kernel<<<blocks, 256, 0, I->stream>>> (I->dEigen + (size_t)eigen * I->eigenStride, tmp, tmp + n2, tmp + 2*n2, S);
-    I->launches++; I->launchKind[MB200_KERNEL_SETUP]++;
+    I->launchKind[MB200_KERNEL_SETUP]++;
     if (I->dFactor)         // the factors are the caller's V and V^-1 themselves
         {
         cudaMemcpyAsync (I->dFactor + (size_t)eigen * 2 * n2, tmp, n2 * sizeof(double), cudaMemcpyDeviceToDevice, I->stream);
@@ -1555,7 +1544,7 @@ int mb200_set_rate_matrices (int instance, int eigen, int like_eigen, const doub
     int blocks = (int)((n3 + 255) / 256); if (blocks > 512) blocks = 512;
     cijk_parts_kernel<<<dim3 (blocks, parts), 256, 0, I->stream>>> (block, vec, S);
     CK (cudaGetLastError ());
-    I->launches += 3; I->launchKind[MB200_KERNEL_SETUP] += 3;
+    I->launchKind[MB200_KERNEL_SETUP] += 3;
     return MB200_SUCCESS;
 }
 
@@ -1766,10 +1755,12 @@ int mb200_set_transition_matrix (int instance, int matrix, const float *in)
     CK (cudaMemcpyAsync (I->dMatrices + (size_t)matrix * n, in, n * sizeof(float), cudaMemcpyHostToDevice, I->stream));
     if (I->tcS)
         {
-        dim3 sg (1, I->cfg.category_count);
-        if (I->tcS == 61) tc_split_kernel<61><<<sg, 128, 0, I->stream>>> (I->dMatrices, I->dSplit, nullptr, matrix, I->cfg.category_count);
-        else              tc_split_kernel<20><<<sg, 128, 0, I->stream>>> (I->dMatrices, I->dSplit, nullptr, matrix, I->cfg.category_count);
-        I->launches++; I->launchKind[MB200_KERNEL_SETUP]++;
+        const int K = I->cfg.category_count;
+        withTcS (I->tcS, [&] (auto s)
+            {
+            tc_split_kernel<decltype (s)::value><<<dim3 (1, K), 128, 0, I->stream>>> (I->dMatrices, I->dSplit, nullptr, matrix, K);
+            });
+        I->launchKind[MB200_KERNEL_SETUP]++;
         }
     CK (cudaStreamSynchronize (I->stream));
     return MB200_SUCCESS;
@@ -1812,7 +1803,6 @@ int mb200_pack_evaluations (int instance, const mb200_evaluation *evaluations, i
     if (cudaMemcpyAsync (b->dBlob, b->hBlob, b->bytes, cudaMemcpyHostToDevice, I->stream) != cudaSuccess ||
         cudaStreamSynchronize (I->stream) != cudaSuccess)
         { freeBatch (*b); delete b; return MB200_ERROR_CUDA; }
-    b->used = true;
     for (size_t i = 0; i < I->batches.size (); i++)
         if (I->batches[i] == nullptr) { I->batches[i] = b; *batch = (int) i; return MB200_SUCCESS; }
     I->batches.push_back (b);
@@ -1829,7 +1819,7 @@ int mb200_replay (int instance, int batch)
     Batch &rb = *I->batches[batch];
     if (rb.tipEpoch != I->tipEpoch)
         return MB200_ERROR_OUT_OF_RANGE;           // tip states changed since mb200_pack_evaluations: pack again
-    return launch (I, rb, rb.dRes, false);
+    return launch (I, rb, false, false);
 }
 
 int mb200_replay_begin (int instance, int batch)
@@ -1837,25 +1827,16 @@ int mb200_replay_begin (int instance, int batch)
     Instance *I = get (instance);
     if (!I) return MB200_ERROR_BAD_INSTANCE;
     if (batch < 0 || batch >= (int) I->batches.size () || !I->batches[batch]) return MB200_ERROR_OUT_OF_RANGE;
-    if (I->pendingCount > 0) return MB200_ERROR_OUT_OF_RANGE;       // one evaluation in flight per instance
+    if (I->pending.count > 0) return MB200_ERROR_OUT_OF_RANGE;      // one evaluation in flight per instance
     CK (cudaSetDevice (I->cfg.device));                               // not use (): a resident kernel stays
     Batch &rb = *I->batches[batch];
     if (rb.tipEpoch != I->tipEpoch)
         return MB200_ERROR_OUT_OF_RANGE;
-    int rc;
     if (residentEligible (I, rb))
-        rc = residentStart (I, rb);
-    else
-        {
-        rc = retire (I);
-        if (rc != MB200_SUCCESS) return rc;
-        I->lastHostSum = 0; I->lastTiles = 1;
-        rc = launch (I, rb, rb.hResDev, false, rb.allRoot && rb.fused);
-        I->pendingSeq = I->seq; I->pendingResident = false;
-        }
+        return residentStart (I, rb);
+    int rc = retire (I);
     if (rc != MB200_SUCCESS) return rc;
-    I->pendingCount = rb.nEval; I->pendingBatch = &rb;
-    return MB200_SUCCESS;
+    return launch (I, rb, false, true);
 }
 
 int mb200_replay_end (int instance, double *lnL, int *status)
@@ -1918,7 +1899,8 @@ int mb200_get_launch_count (int instance, long long *launches)
 {
     Instance *I = get (instance);
     if (!I || !launches) return MB200_ERROR_BAD_INSTANCE;
-    *launches = I->launches;
+    *launches = 0;
+    for (long long n : I->launchKind) *launches += n;
     return MB200_SUCCESS;
 }
 

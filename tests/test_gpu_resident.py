@@ -106,6 +106,30 @@ def test_other_calls_between_generations(engine_lib, launched):
     assert all(np.array_equal(a, b) for a, b in zip(scal, launched[2]))
 
 
+def test_replay_between_begin_and_end(engine_lib, launched):
+    """A synchronous mb200_replay (results to device memory) while a replay_begin is pending must not change
+    how replay_end collects the pending results: the tile partials are still summed on the host."""
+    job = bench.Job("primates", 0, 1, engine_lib, 0, CYCLE)
+    try:
+        inst = job.insts[0]
+        batches = [inst.pack(job.steps[0][i]) for i in range(CYCLE)]
+        lnls = []
+        for g in range(CYCLE):
+            b = batches[g]
+            assert engine_lib.fn("replay_begin")(inst.handle, b) == 0
+            if g % 4 == 1:
+                inst.replay(b)                        # the same evaluation again: same inputs, same outputs
+            lnl = np.zeros(8, np.float64)
+            st = np.zeros(8, np.int32)
+            assert engine_lib.fn("replay_end")(inst.handle, lnl.ctypes.data_as(C.POINTER(C.c_double)),
+                                               st.ctypes.data_as(C.POINTER(C.c_int))) == 0
+            assert not st.any()
+            lnls.append(lnl)
+    finally:
+        job.close()
+    assert np.array_equal(np.array(lnls), launched[0][:CYCLE])
+
+
 def test_second_instance_falls_back_to_launches(engine_lib, launched):
     other = workloads.make_problem(4, 4, 64, 8, 1, seed=3)
     with other.create(engine_lib):
