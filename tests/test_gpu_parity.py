@@ -85,13 +85,18 @@ CASES = [
     (4, 3, 500, 8, 0.0, 0.05),
     (4, 5, 77, 5, 0.0, 0.0),
     (4, 8, 260, 6, 0.3, 0.0),
+    (4, 6, 97, 7, 0.1, 0.05),
+    (4, 7, 64, 9, 0.0, 0.0),
     (4, 10, 60, 5, 0.0, 0.0),      # K > 8: generic kernel on 4 states
     (20, 4, 88, 9, 0.0, 0.0),
     (20, 4, 33, 6, 0.1, 0.2),
     (20, 1, 70, 5, 0.0, 0.0),
+    (20, 2, 129, 8, 0.0, 0.1),
+    (20, 3, 128, 7, 0.15, 0.0),
     (61, 1, 239, 9, 0.0, 0.0),
     (61, 1, 20, 4, 0.0, 0.1),
     (61, 2, 31, 5, 0.0, 0.0),
+    (61, 3, 130, 6, 0.0, 0.0),     # the NY98 / M3 shape: three omega categories
     (2, 4, 50, 6, 0.0, 0.0),
     (16, 2, 45, 6, 0.0, 0.0),
     (64, 1, 19, 5, 0.0, 0.0),
@@ -243,6 +248,24 @@ def test_time_min_and_time_max_branches(engine_lib, oracle_lib):
         assert rel(le, lo) < LNL_RTOL
         P0 = e.get_transition_matrix(int(pr.chains[0].ti[0]))
         assert np.array_equal(P0, np.broadcast_to(np.eye(4, dtype=np.float32), P0.shape))
+        P1 = e.get_transition_matrix(int(pr.chains[0].ti[1]))
+        assert np.array_equal(P1, np.broadcast_to(pr.freqs.astype(np.float32)[None, None, :], P1.shape))
+
+
+@pytest.mark.parametrize("S,K", [(16, 4), (20, 4), (61, 3), (61, 4), (64, 2)])
+def test_time_min_and_time_max_branches_other_state_counts(engine_lib, oracle_lib, S, K):
+    """The same limits in the other P(t) builders: tiprobs_kernel (16 states; 20 states, then the
+    tensor-core split images) and tiprobs_mm_kernel (61 and 64 states)."""
+    pr = workloads.make_problem(S, K, 50, 6, 1, seed=3)
+    pr.tree[0].length[0] = 1e-13
+    pr.tree[0].length[1] = 5000.0
+    with pr.create(engine_lib) as e, pr.create(oracle_lib) as o:
+        o.set_arith(1)
+        sp = pr.full_evaluation(0)
+        (le,), _ = e.evaluate(sp); (lo,), _ = o.evaluate(sp)
+        assert rel(le, lo) < lnl_tol(S, SYN_RTOL)
+        P0 = e.get_transition_matrix(int(pr.chains[0].ti[0]))
+        assert np.array_equal(P0, np.broadcast_to(np.eye(S, dtype=np.float32), P0.shape))
         P1 = e.get_transition_matrix(int(pr.chains[0].ti[1]))
         assert np.array_equal(P1, np.broadcast_to(pr.freqs.astype(np.float32)[None, None, :], P1.shape))
 
