@@ -105,17 +105,20 @@ struct JobIndex
 // pinned, mapped host memory, and every piece carries the job's sequence number in .w, so a reader
 // that finds the same number in every piece it read has an untorn job.
 //   piece 0: count (MB200_RES_STOP: exit), blob address lo, hi     piece 1: result address lo, hi, offEval
-//   piece 2: offDbl, offChunk, offCmat                             piece 3: offOp
+//   piece 2: offDbl, offChunk, offCmat                             piece 3: offOp, (device copy only) done target
 //   piece 4 + 2e, 5 + 2e: JobIndexEntry of evaluation e (matOff, nMat, opOff | nOp, dOff, eigen0)
 #define MB200_RES_HEAD   4
 #define MB200_RES_PIECES (MB200_RES_HEAD + 2 * MB200_JOB_INDEX_MAX)
+#define MB200_RES_ROW    (MB200_RES_HEAD + 2)
 #define MB200_RES_STOP   0x7fffffff
-struct ResidentJob                  // device memory: the leader CTA's copy of the current job for the others
+struct ResidentJob                  // device memory, written by the leader CTA for the others
 {
-    unsigned long long word;        // sequence number << 32 | count (MB200_RES_STOP: exit)
     unsigned int ack;               // jobs seen, summed over the CTAs (monotone, wraps)
-    unsigned int pad;
-    int4 piece[MB200_RES_PIECES];
+    unsigned int done;              // jobs finished, summed over the CTAs that ran them (monotone, wraps); a CTA adds
+                                    // its 1 after its writes, so a count reached releases every write before it
+    unsigned int pad[2];
+    int4 row[MB200_JOB_INDEX_MAX][MB200_RES_ROW];   // per evaluation row: the job's header pieces and the row's two
+                                                    // JobIndexEntry pieces, each with the sequence number in .w
 };
 
 // evaluations with at most this many pattern tiles add their tile partials left to right -- on the
