@@ -10,15 +10,23 @@ TIME_MIN = float(np.float32(1.0e-11))       # P(t) = I below, stationary rows ab
 TIME_MAX = float(np.float32(100.0))
 
 
-def transition_matrices(pr, length, rates):
-    """[K, S, S] P(t) = V diag(exp(lambda r_k t)) V^-1 in double, negative entries clamped to 0."""
+def transition_matrices(pr, length, rates, Q=None, freqs=None):
+    """[K, S, S] P(t) in double, negative entries clamped to 0: V diag(exp(lambda r_k t)) V^-1 from the
+    problem's eigensystem, or with Q -- [S, S], or [K, S, S], one rate matrix per category -- the matrix
+    exponential expm(Q_k r_k t), independent of any eigensystem.  Stationary rows are `freqs` (default
+    the problem's)."""
+    from scipy.linalg import expm
+    freqs = np.asarray(pr.freqs if freqs is None else freqs, float)
+    Qk = None if Q is None else np.broadcast_to(np.asarray(Q, float).reshape(-1, pr.S, pr.S), (len(rates), pr.S, pr.S))
     out = []
-    for r in rates:
+    for k, r in enumerate(rates):
         t = length * r
         if t < TIME_MIN:
             out.append(np.eye(pr.S))
         elif t > TIME_MAX:
-            out.append(np.tile(np.asarray(pr.freqs, float), (pr.S, 1)))
+            out.append(np.tile(freqs, (pr.S, 1)))
+        elif Qk is not None:
+            out.append(np.maximum(expm(Qk[k] * t), 0.0))
         else:
             out.append(np.maximum((pr.V * np.exp(pr.lam * t)) @ pr.Vinv, 0.0))
     return np.array(out)
@@ -30,39 +38,49 @@ def tip_partials(pr, tip):
     return bits.astype(np.float64)
 
 
-def f64_lnl(pr, ch, tree=None):
-    """-> (per-pattern log likelihoods [C], lnL) of chain `ch` on its current tree."""
+def f64_lnl(pr, ch, tree=None, *, Q=None, freqs=None, rates=None, cat_weights=None, p_invar=None, weights=None):
+    """-> (per-pattern log likelihoods [C], lnL) of chain `ch` on its current tree.
+
+    Without overrides the model is the problem's: its eigensystem, frequencies, rates / (1 - p_invar) and
+    equal category weights (1 - p_invar) / K.  Overrides describe one evaluation's own model: Q (per-category
+    rate matrices, see transition_matrices), freqs, rates and cat_weights exactly as the evaluation sends
+    them, p_invar (0: none) and the pattern weights of its weights row."""
     tr = pr.tree[ch] if tree is None else tree
-    rates = np.asarray(pr.rates, float) / (1.0 - pr.p_invar)
-    catw = (1.0 - pr.p_invar) / pr.K
+    pinv = pr.p_invar if p_invar is None else float(p_invar)
+    freqs = np.asarray(pr.freqs if freqs is None else freqs, float)
+    rates = np.asarray(pr.rates, float) / (1.0 - pinv) if rates is None else np.asarray(rates, float)
+    catw = np.full(pr.K, (1.0 - pinv) / pr.K) if cat_weights is None else np.asarray(cat_weights, float)
+    weights = np.asarray(pr.weights if weights is None else weights, float)
     cl, lnscale = {}, np.zeros(pr.C)
+
+    def pmat(node):
+        return transition_matrices(pr, tr.length[node], rates, Q, freqs)
 
     def child(node):
         x = np.broadcast_to(tip_partials(pr, node), (pr.K, pr.C, pr.S)) if node < tr.n_tips else cl[node]
-        P = transition_matrices(pr, tr.length[node], rates)
-        return np.einsum("kij,kcj->kci", P, x)
+        return np.einsum("kij,kcj->kci", pmat(node), x)
 
     for p in tr.post:
         x = child(int(tr.left[p])) * child(int(tr.right[p]))
         if tr.anc[p] == tr.root:                       # the interior root also takes the root tip
             rt = tip_partials(pr, tr.root)[None]
-            x = x * np.einsum("kij,kcj->kci", transition_matrices(pr, tr.length[p], rates), np.broadcast_to(rt, x.shape))
+            x = x * np.einsum("kij,kcj->kci", pmat(p), np.broadcast_to(rt, x.shape))
         m = x.max(axis=(0, 2))
         m = np.where(m > 0, m, 1.0)
         cl[p] = x / m[None, :, None]
         lnscale += np.log(m)
-    like = catw * np.einsum("kcs,s->c", cl[tr.root_left], np.asarray(pr.freqs, float))
-    if pr.p_invar > 0:
+    like = np.einsum("k,kcs,s->c", catw, cl[tr.root_left], freqs)
+    if pinv > 0:
         inv = np.bitwise_and.reduce(pr.masks, axis=0)
         bits = (inv[:, None] >> np.arange(pr.S, dtype=np.uint64)[None, :]) & np.uint64(1)
-        like_i = pr.p_invar * (bits * np.asarray(pr.freqs, float)[None, :]).sum(1)
+        like_i = pinv * (bits * freqs[None, :]).sum(1)
         # Likelihood_Gen's formula; below a scaler of -200 the reference switches to an approximation
         assert lnscale.min() >= -200.0, "site scaler below -200: the reference approximates there"
         site = lnscale + np.log(like + like_i * np.exp(-lnscale))
     else:
         with np.errstate(divide="ignore"):
             site = lnscale + np.log(like)
-    return site, float(site @ np.asarray(pr.weights, float))
+    return site, float(site @ weights)
 
 
 # ----------------------------------------------------------------------------- trees

@@ -85,3 +85,67 @@ def test_f64_transition_matrix_limits(S):
     from scipy.linalg import expm
     Q = (pr.V * pr.lam) @ pr.Vinv
     assert np.allclose(P[1], expm(Q * 0.3), atol=1e-12)
+
+
+# ---- per-chain models (tests/chain_models.py): the oracle paths the shared-model cases never take -----------
+MIXED_CASES = [
+    # S, K, parts, C, tips, chains
+    (4, 4, 1, 150, 12, 4),          # unequal category weights at S = 4 (the oracle's non-`equal` root), inline
+    (4, 7, 1, 97, 9, 4),            # eigensystems next to slot ones, weights rows 1..3
+    (61, 3, 3, 15, 6, 3),           # one Q per omega category (MB200_CONFIG_CIJK_PARTS(3))
+    (20, 2, 1, 40, 7, 3),
+    (16, 5, 1, 33, 8, 3),
+]
+
+
+@pytest.mark.parametrize("S,K,parts,C,tips,nch", MIXED_CASES)
+def test_f64_reference_per_chain_models(oracle_lib, S, K, parts, C, tips, nch):
+    """Every chain with its own slot (slot 0 a decoy), frequencies, rates, category weights, p_invar, flags and
+    weights row (row 0 a decoy): the float64 reference with the evaluation's own model against the oracle, after
+    a full evaluation and after branch updates; and the models differ enough to tell an index mix-up."""
+    from chain_models import MixedModels
+    pr = workloads.make_problem(S, K, C, tips, nch, seed=500 + S + K, p_ambig=0.0)
+    pr.tree[0] = caterpillar_tree(tips, np.random.default_rng(S))
+    mm = MixedModels(pr, seed=S * K)
+    ms = mm.models
+    assert {m.slot for m in ms} == set(range(1, nch + 1)) and all(m.row > 0 for m in ms)
+    assert len({m.row for m in ms}) > 1 and any(m.p_invar > 0 for m in ms) and any(m.p_invar == 0 for m in ms)
+    if K > 1:
+        assert any(np.ptp(m.cat_weights) > 0 for m in ms) and any(np.ptp(m.cat_weights) == 0 for m in ms)
+    if S == 4:
+        assert any(m.inline for m in ms) and not all(m.inline for m in ms)
+    rng = np.random.default_rng(S)
+    with mm.create(oracle_lib) as o, mm.create(oracle_lib) as scratch:
+        o.set_arith(1)
+        scratch.set_arith(1)
+        mm.assert_models_differ(scratch, range(nch))
+        for ch in range(nch):
+            (lo,), (so,) = o.evaluate(mm.full(ch))
+            assert so == abi.EVAL_OK
+            lf = mm.f64(ch)
+            assert abs(lo - lf) < RTOL * abs(lf), f"chain {ch}"
+        for it in range(2 * nch):
+            ch = it % nch
+            old = pr.tree[ch].length.copy()
+            sp = mm.update(ch, rng)
+            (lo,), _ = o.evaluate(sp)
+            lf = mm.f64(ch)
+            assert abs(lo - lf) < RTOL * abs(lf), f"update {it}"
+            if it % 3 == 2:
+                pr.reject(ch, sp, old)
+        # root integration alone under another weights row and p_invar: the same buffers, other sums
+        m = ms[1].with_p_invar(0.2).replace(row=1 + ms[1].row % (mm.rows - 1))
+        (lo,), _ = o.evaluate(mm.apply(mm.root_only(1), m))
+        lf = mm.f64(1, m)
+        assert abs(lo - lf) < RTOL * abs(lf)
+
+
+def test_f64_reference_matrix_exponential_matches_eigensystem():
+    """the Q override builds P(t) by expm: the same matrices as the problem's eigensystem, limits included"""
+    pr = workloads.make_problem(4, 3, 5, 4, 1, seed=2)
+    Q = (pr.V * pr.lam) @ pr.Vinv
+    rates = np.array([0.3, 1.0, 2.5])
+    for t in (1e-13, 0.05, 0.7, 5000.0):
+        assert np.allclose(transition_matrices(pr, t, rates, Q=Q), transition_matrices(pr, t, rates), atol=1e-12)
+    Qs = np.stack([Q, 2 * Q, 3 * Q])
+    assert np.allclose(transition_matrices(pr, 0.2, np.ones(3), Q=Qs), transition_matrices(pr, 0.2, [1.0, 2.0, 3.0]), atol=1e-12)
