@@ -83,6 +83,104 @@ def f64_lnl(pr, ch, tree=None, *, Q=None, freqs=None, rates=None, cat_weights=No
     return site, float(site @ weights)
 
 
+# ----------------------------------------------------------------------------- variable-state (Std) divisions
+BRLENS_MIN = float(np.float32(1e-8))        # TiProbs_Std clamps the branch length to [BRLENS_MIN, BRLENS_MAX]
+BRLENS_MAX = float(np.float32(100.0))
+LIKE_EPSILON = 1e-300
+
+
+def mk_rate_matrix(n):
+    """Q of the equal-frequency Mk model on n states: 1/(n-1) off the diagonal, -1 on it (one change per unit time)"""
+    Q = np.full((n, n), 1.0 / (n - 1))
+    np.fill_diagonal(Q, -1.0)
+    return Q
+
+
+def std_pattern_classes(pr):
+    """-> [(n, tiIndex, pattern indices)], one entry per (state count, matrix offset) pair"""
+    keys = sorted(set(zip(pr.state_counts.tolist(), pr.matrix_offsets.tolist())))
+    return [(n, ti, np.flatnonzero((pr.state_counts == n) & (pr.matrix_offsets == ti))) for n, ti in keys]
+
+
+class StdLnl:
+    """f64_std_lnl's result: per-pattern log likelihoods (site), lnL, the probability of the unobservable
+    (dummy) patterns p_un, and whether a non-dummy pattern's likelihood fell below LIKE_EPSILON"""
+
+    def __init__(self, site, lnl, p_un, underflow):
+        self.site, self.lnl, self.p_un, self.underflow = site, lnl, p_un, underflow
+
+    def bound(self, pr, weights=None):
+        """|lnL - lnL64| allowed for a float evaluation: 2e-7 relative on every observed pattern's log term, plus the
+        conditioning of the coding-bias correction, U * 2e-6 * pUn / pObserved (float partials carry a few ulps into
+        pUn; the log divides by pObserved).  When 1 - pUn is below LIKE_EPSILON the correction is the clamped
+        constant on every side and adds nothing."""
+        w = np.asarray(pr.weights if weights is None else weights, float)[pr.dummy:]
+        return 2e-7 * float(np.abs(self.site[pr.dummy:]) @ w) + self.conditioning(pr)
+
+    def conditioning(self, pr):
+        """U * 2e-6 * pUn / pObserved, or 0 without dummies or when the correction is clamped"""
+        p_obs = 1.0 - self.p_un
+        return pr.uncompressed * 2e-6 * self.p_un / p_obs if pr.dummy and p_obs >= LIKE_EPSILON else 0.0
+
+
+def f64_std_lnl(pr, ch, tree=None, *, rates=None, matrices=None, weights=None):
+    """Float64 likelihood of a variable-state (STANDARD data) division, from the model's definition.
+
+    Pattern c has n = state_counts[c] states.  P(t) of category k is expm(Q_n v) with v = clamp(length, BRLENS_MIN,
+    BRLENS_MAX) * r_k, or, for a branch in `matrices` (node -> the branch's block of matrix_length floats in the host
+    layout), the block's [n][n] matrix at matrix_offsets[c] + k n^2, read as row a (parent state), column i (child
+    state).  Pruning with the interior root's three neighbours and per-pattern rescaling by the max over categories
+    and states.  At the root L_c = 1/K sum_k sum_j pi_j cl[k][c][j], pi = freqs[freq_offsets[c]:] (category weights
+    are not used), and lnL = sum_{c >= dummy} w_c log L_c - U log(max(1 - sum_{c < dummy} L_c, LIKE_EPSILON)).
+    -> StdLnl"""
+    from scipy.linalg import expm
+    tr = pr.tree[ch] if tree is None else tree
+    rates = np.asarray(pr.rates if rates is None else rates, float)
+    weights = np.asarray(pr.weights if weights is None else weights, float)
+    matrices = matrices or {}
+    K = len(rates)
+    classes = std_pattern_classes(pr)
+    lnscale = np.zeros(pr.C)
+    cl = {}                                              # (node, class) -> [K, patterns, n]
+
+    def pmat(node, n, ti):
+        if node in matrices:
+            blk = np.asarray(matrices[node], np.float64)
+            return blk[ti:ti + K * n * n].reshape(K, n, n)
+        v = min(max(float(tr.length[node]), BRLENS_MIN), BRLENS_MAX) * rates
+        return np.array([expm(mk_rate_matrix(n) * vk) for vk in v])
+
+    def tip(node, idx, n):
+        m = pr.masks[node][idx]
+        return ((m[:, None] >> np.arange(n, dtype=np.uint64)[None, :]) & np.uint64(1)).astype(np.float64)
+
+    def child(node, j, n, ti, idx):
+        x = np.broadcast_to(tip(node, idx, n), (K, len(idx), n)) if node < tr.n_tips else cl[node, j]
+        return np.einsum("kai,kci->kca", pmat(node, n, ti), x)
+
+    for p in tr.post:
+        l, r = int(tr.left[p]), int(tr.right[p])
+        for j, (n, ti, idx) in enumerate(classes):
+            x = child(l, j, n, ti, idx) * child(r, j, n, ti, idx)
+            if tr.anc[p] == tr.root:                     # the interior root also takes the root tip
+                x = x * np.einsum("kai,kci->kca", pmat(p, n, ti), np.broadcast_to(tip(tr.root, idx, n), x.shape))
+            m = x.max(axis=(0, 2))
+            m = np.where(m > 0, m, 1.0)
+            cl[p, j] = x / m[None, :, None]
+            lnscale[idx] += np.log(m)
+    like = np.zeros(pr.C)
+    for j, (n, ti, idx) in enumerate(classes):
+        pi = pr.freqs[pr.freq_offsets[idx][:, None] + np.arange(n)[None, :]]      # [patterns, n]
+        like[idx] = np.einsum("kcj,cj->c", cl[tr.root_left, j], pi) / K
+    d = pr.dummy
+    underflow = bool((like[d:] < LIKE_EPSILON).any())
+    with np.errstate(divide="ignore"):
+        site = lnscale + np.log(like)
+    p_un = float((like[:d] * np.exp(lnscale[:d])).sum())
+    lnl = float(site[d:] @ weights[d:]) - pr.uncompressed * np.log(max(1.0 - p_un, LIKE_EPSILON))
+    return StdLnl(site, lnl, p_un, underflow)
+
+
 # ----------------------------------------------------------------------------- trees
 def tree_height(tr, node=None):
     """interior levels from the tips up to `node` (default: the interior root)"""

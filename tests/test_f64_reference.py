@@ -1,7 +1,7 @@
 """CPU: the float64 pruning reference against the CPU oracle, on the synthetic configurations the
 recorded reference runs (tests/golden) do not cover -- 2, 16, 40 and 64 states, 6 and 7 rate
-categories -- so that the oracle, the only judge of the engine there, is itself checked; and the
-tree builders the GPU path tests use."""
+categories, and variable-state (Std) divisions at the shapes of test_gpu_std.py -- so that the oracle, the
+only judge of the engine there, is itself checked; and the tree builders the GPU path tests use."""
 import numpy as np
 import pytest
 
@@ -149,3 +149,140 @@ def test_f64_reference_matrix_exponential_matches_eigensystem():
         assert np.allclose(transition_matrices(pr, t, rates, Q=Q), transition_matrices(pr, t, rates), atol=1e-12)
     Qs = np.stack([Q, 2 * Q, 3 * Q])
     assert np.allclose(transition_matrices(pr, 0.2, np.ones(3), Q=Qs), transition_matrices(pr, 0.2, [1.0, 2.0, 3.0]), atol=1e-12)
+
+
+# ---- variable-state (Std) divisions: the float64 reference against the oracle at the shapes of test_gpu_std.py ----
+def std_oracle_run(oracle_lib, name, updates=6):
+    """-> [(evaluation, oracle lnL, oracle status, float64 StdLnl)] of a full evaluation per chain and branch updates"""
+    from f64_reference import f64_std_lnl
+    from std_problems import make_case, run_specs
+    pr, supplier = make_case(name)
+    out = []
+    with pr.create(oracle_lib) as o:
+        for sp in run_specs(pr, updates, seed=1):
+            if supplier:
+                supplier(sp, [o])
+            (lo,), (so,) = o.evaluate(sp)
+            ref = f64_std_lnl(pr, sp.chain, rates=pr.chain_rates[sp.chain],
+                              matrices=supplier.matrices(sp.chain) if supplier else None)
+            out.append((sp, lo, so, ref))
+    return pr, out
+
+
+def _std_case_names():
+    from std_problems import CASES
+    return list(CASES)
+
+
+@pytest.mark.parametrize("name", _std_case_names())
+def test_f64_std_reference_matches_oracle(oracle_lib, name):
+    """Mk (or caller-supplied) matrices per state-count class, per-chain rates, the coding-bias correction: lnL within
+    2e-7 relative; the clamp case is -U log(1e-300) on both; nothing underflows"""
+    pr, out = std_oracle_run(oracle_lib, name)
+    for i, (sp, lo, so, ref) in enumerate(out):
+        assert so == abi.EVAL_OK and not ref.underflow, f"evaluation {i}"
+        # near-degenerate: the float partials' ulps in pUn ~ 1 become relative errors of pObserved ~ 1e-4
+        assert abs(lo - ref.lnl) < RTOL * abs(ref.lnl) + ref.conditioning(pr), f"evaluation {i}: {lo!r} vs {ref.lnl!r}"
+    if name == "clamp":
+        assert ref.p_un > 1.9
+    if name == "near-degenerate":
+        assert all(1e-5 < 1.0 - r.p_un < 1e-3 for *_, r in out)
+    if name.startswith("informative"):
+        assert pr.dummy == 66
+
+
+def test_f64_std_reference_orientation(oracle_lib):
+    """The non-symmetric matrices decide the result: reading them transposed moves lnL far outside the tolerance"""
+    from f64_reference import f64_std_lnl, std_pattern_classes
+    from std_problems import make_case
+    pr, supplier = make_case("supplied-nonsymmetric-K3")
+    with pr.create(oracle_lib) as o:
+        sp = supplier(pr.full_evaluation(0), [o])
+        (lo,), _ = o.evaluate(sp)
+    mats = supplier.matrices(0)
+    ref = f64_std_lnl(pr, 0, rates=pr.chain_rates[0], matrices=mats)
+    transposed = {}
+    for node, blk in mats.items():
+        t = blk.copy()
+        for n, ti, _ in std_pattern_classes(pr):
+            for k in range(pr.K):
+                s = slice(ti + k * n * n, ti + (k + 1) * n * n)
+                t[s] = blk[s].reshape(n, n).T.ravel()
+        transposed[node] = t
+    wrong = f64_std_lnl(pr, 0, rates=pr.chain_rates[0], matrices=transposed)
+    assert abs(lo - ref.lnl) < RTOL * abs(ref.lnl)
+    assert abs(wrong.lnl - ref.lnl) > 1e3 * RTOL * abs(ref.lnl)
+
+
+def test_f64_std_reference_matrices_and_layout():
+    """Mk by expm against its closed form (TiProbs_Std); ordered matrices symmetric birth-death chains; the tables
+    of an ordered, informative division in the reference's layout"""
+    from scipy.linalg import expm
+    from f64_reference import mk_rate_matrix
+    from std_problems import dummy_masks, make_std_division, ordered_rate_matrix
+    for n in (2, 3, 7, 24):
+        v = 0.37
+        e = np.exp(-n / (n - 1) * v)
+        P = expm(mk_rate_matrix(n) * v)
+        assert np.allclose(np.diag(P), 1 / n + (n - 1) / n * e, atol=1e-14)
+        assert np.allclose(P[0, 1:], 1 / n - e / n, atol=1e-14)
+        Q = ordered_rate_matrix(n)
+        assert np.allclose(Q.sum(1), 0) and np.isclose(-np.diag(Q).mean(), 1.0) and np.allclose(Q, Q.T)
+        assert np.count_nonzero(np.triu(Q, 2)) == 0
+    dm = dummy_masks(4, "informative")
+    assert dm.shape == (4, 10) and list(dm[:, 0]) == [2, 1, 1, 1] and list(dm[:, 4]) == [1, 2, 2, 2]
+    assert list(dm[:, 8]) == [1] * 4 and list(dm[:, 9]) == [2] * 4
+    pr = make_std_division(60, 3, 5, 1, seed=1, states=(2, 3, 5), ordered=(3, 5), coding="informative")
+    assert pr.dummy == 12 and pr.weights[:12].sum() == 0 and pr.uncompressed == int(pr.weights.sum())
+    blocks = [(2, False), (3, False), (5, False), (3, True), (5, True)]
+    ti = np.cumsum([0] + [n * n * 3 for n, _ in blocks])
+    bs = np.cumsum([0] + [n for n, _ in blocks])
+    for c in range(pr.C):
+        j = blocks.index((int(pr.state_counts[c]), bool(pr.ordered[c])))
+        assert pr.matrix_offsets[c] == ti[j] and pr.freq_offsets[c] == bs[j]
+    assert pr.matrix_length == ti[-1] and len(pr.freqs) == bs[-1]
+
+
+def tree_from_evaluation(sp, n_tips):
+    """The tree of a full evaluation (every branch's matrix update, every interior node's operation), in MrBayes'
+    numbering: interior node n_tips + i is the destination of operation i, the root tip is the last one's third child"""
+    length = {int(m["matrix"]): float(m["length"]) for m in sp.mats}
+    n_nodes = 2 * n_tips - 2
+    left, right, anc, lens = np.full(n_nodes, -1), np.full(n_nodes, -1), np.full(n_nodes, -1), np.zeros(n_nodes)
+    node = {}
+    for i, op in enumerate(sp.ops):
+        p = n_tips + i
+        node[int(op["dest"])] = p
+        for side, (c, m) in enumerate(((op["child1"], op["matrix1"]), (op["child2"], op["matrix2"]))):
+            cn = int(c) if c < n_tips else node[int(c)]
+            (left if side == 0 else right)[p] = cn
+            anc[cn], lens[cn] = p, length[int(m)]
+        if op["child3"] >= 0:
+            root = int(op["child3"])
+            anc[p], left[root], lens[p] = root, p, length[int(op["matrix3"])]
+    assert len(sp.ops) == n_tips - 2 and len(sp.mats) == n_nodes - 1
+    return workloads.Tree(n_tips, left, right, anc, lens, root, list(range(n_tips, n_nodes)))
+
+
+def test_f64_std_reference_matches_cynmix_golden():
+    """cynmix's morphology partition (Mk + G4, coding=variable): every full evaluation of the recorded reference
+    run, rebuilt as a tree, against the lnL the reference's own Likelihood_Std returned"""
+    from types import SimpleNamespace
+    from conftest import GOLDEN
+    from f64_reference import f64_std_lnl
+    from mrbayes_b200 import records
+    divs, events = records.load(GOLDEN / "cynmix_full_fma.gold.gz")
+    (div,) = [d for d in divs.values() if d.pattern_states is not None]
+    ps, n_tips = div.pattern_states, div.cfg["tip_count"]
+    fulls = [ev.spec for ev in events if ev.kind == "eval" and ev.division == div.division
+             and ev.spec.site_src == abi.NONE and len(ev.spec.ops) == n_tips - 2]
+    assert len(fulls) >= 4
+    masks = np.stack([div.tips[t] for t in range(n_tips)])
+    for sp in fulls:
+        pr = SimpleNamespace(C=div.cfg["pattern_count"], masks=masks, freqs=sp.freqs, weights=div.weights[sp.weights_row],
+                             state_counts=ps["state_counts"], matrix_offsets=ps["matrix_offsets"],
+                             freq_offsets=ps["freq_offsets"], dummy=ps["dummy_patterns"],
+                             uncompressed=ps["uncompressed_sites"])
+        ref = f64_std_lnl(pr, sp.chain, tree_from_evaluation(sp, n_tips), rates=sp.rates)
+        assert not ref.underflow and 0.0 < ref.p_un < 1.0
+        assert abs(ref.lnl - sp.lnl_ref) < RTOL * abs(sp.lnl_ref), f"chain {sp.chain}: {ref.lnl!r} vs {sp.lnl_ref!r}"
