@@ -40,7 +40,6 @@ struct DevEval                      // one LaunchLogLikeForDivision (96 bytes)
     int    equalWeights;
     int    dOff;                    // doubles [dOff ...): rates[K], catW[K], freqs[S]
     double pInvar;
-    int    fuseP;                   // 1: the pruning kernel rebuilds this evaluation's P(t) itself
     int    nChunk;                  // 4-state path: chunk0 below + (nChunk-1) entries at chunkOff
     int    eigen0;                  // eigen slot of the first matrix update (normally of all of them);
                                     // -2: the evaluation carries its own cijk block after freqs in the doubles
@@ -49,6 +48,19 @@ struct DevEval                      // one LaunchLogLikeForDivision (96 bytes)
     int    rootFwd;                 // 4-state path: the root buffer is the last node's result
     unsigned rootOff;               // 4-state path: float4 index of the root buffer
 };
+// the 4-state kernel stages a header as sizeof(DevEval)/4 words, and bench.py counts 96 bytes per evaluation
+static_assert (sizeof(DevEval) == 96, "DevEval must stay 96 bytes");
+
+// the evaluation whose matrix-update list holds update u (matOff is non-decreasing; empty lists are skipped)
+__device__ __forceinline__ int owning_eval (const DevEval *evals, int nEval, int u)
+{
+    int e = 0;
+    while (e + 1 < nEval && u >= evals[e + 1].matOff)
+        e++;
+    while (e > 0 && evals[e].nMat == 0)
+        e--;
+    return e;
+}
 
 struct DevMat                       // one branch (16 bytes)
 {
@@ -121,10 +133,6 @@ struct ResidentJob                  // device memory, written by the leader CTA 
                                                     // JobIndexEntry pieces, each with the sequence number in .w
 };
 
-// evaluations with at most this many pattern tiles add their tile partials left to right -- on the
-// device (last CTA) or, on the host-call latency path, on the host: the same order, the same bits
-#define MB200_SEQ_SUM_TILES 16
-
 // chunk geometry of the 4-state kernels (shared by pack() and the kernels)
 __host__ __device__ constexpr int nuc_maxs (int K)          // P(t) slots per chunk
 {
@@ -140,14 +148,6 @@ __host__ __device__ constexpr int nuc_maxt (int K)
 {
     return (96 / K > 64) ? 64 : 96 / K;
 }
-
-struct DevResult                    // 16 bytes per evaluation
-{
-    double lnL;
-    int    status;
-    int    seq;                     // launch sequence number, written LAST: a host polling the
-                                    // (mapped, pinned) result sees lnL/status complete once seq matches
-};
 
 // Job descriptors handed over as a kernel parameter (constant bank) instead of a host->device
 // copy: removes one stream operation from the latency path of small evaluations.
@@ -179,12 +179,70 @@ struct DevCtx                       // instance geometry + buffer bases, passed 
     const double   *eigen;
     const float    *weights;
     const uint64_t *invMask;
-    double         *tilePartial;    // [maxEval][numTiles] per-tile lnL partial sums
+    double2        *tilePartial;    // [maxEval][numTiles] per-tile lnL partial sum, and (Std) unobserved probability
     int            *tileAbort;      // [maxEval][numTiles]
     unsigned int   *ticket;         // [maxEval]
     int    cijkParts;               // eigensystems per cijk slot: 1, or K (category k uses part k: NY98-type models)
     int    patternTiles;            // 4-state path: tiles of tilePatterns patterns; numTiles (CTAs per evaluation) may be
                                     // smaller: a CTA then walks several tiles (throughput mode)
 };
+
+// ---- cross-tile lnL reduction, shared by every evaluation kernel ----
+// Each tile (CTA, or tensor-core closing item) reduces its patterns' terms itself, then one thread calls
+// tile_arrive; the last tile of the evaluation to arrive adds the partials (tile_sum_ltr, or a strided
+// block sum above MB200_SEQ_SUM_TILES) and writes the evaluation's DevResult with dev_result_write.
+
+// evaluations with at most this many pattern tiles add their tile partials left to right -- on the
+// device (last CTA) or, on the host-call latency path, on the host: the same order, the same bits
+#define MB200_SEQ_SUM_TILES 16
+
+struct DevResult                    // 16 bytes per evaluation
+{
+    double lnL;
+    int    status;
+    int    seq;                     // launch sequence number, written LAST: a host polling the
+                                    // (mapped, pinned) result sees lnL/status complete once seq matches
+};
+
+// one 16-byte store: lnL, status and the sequence number travel in a single write, so a host polling
+// `seq` in (mapped, pinned) memory never sees a half-written result and no system-scope fence sits on
+// the critical path.  The values are written as given (tile packets of the host-sum path included).
+__device__ __forceinline__ void dev_result_write (DevResult *slot, double lnL, int status, int seq)
+{
+    int4 pkt;
+    pkt.x = __double2loint (lnL); pkt.y = __double2hiint (lnL); pkt.z = status; pkt.w = seq;
+    *reinterpret_cast<int4 *>(slot) = pkt;
+}
+
+// one thread of a tile, after the tile's reduction: publish the tile's partial and abort flag, then take
+// the evaluation's ticket.  True for the last of its numTiles tiles to arrive.  (numTiles is ctx.numTiles;
+// a kernel that keeps it in a register passes that, which keeps the tensor-core kernel's spills down.)
+__device__ __forceinline__ bool tile_arrive (const DevCtx &ctx, int evalIdx, int numTiles, int tile, double2 partial, int abortFlag)
+{
+    const size_t slot = (size_t)evalIdx * numTiles + tile;
+    ctx.tilePartial[slot] = partial;
+    ctx.tileAbort[slot] = abortFlag;
+    __threadfence ();
+    return atomicAdd (&ctx.ticket[evalIdx], 1u) == (unsigned int) numTiles - 1u;
+}
+
+struct TileSum { double lnL, unobserved; int abort; };
+
+// the last tile to arrive, one thread: the partials of every tile added left to right, abort flags OR-ed;
+// then the ticket is reset for the next launch
+__device__ __forceinline__ TileSum tile_sum_ltr (const DevCtx &ctx, int evalIdx, int numTiles)
+{
+    __threadfence ();
+    TileSum r = { 0.0, 0.0, 0 };
+    for (int t = 0; t < numTiles; t++)
+        {
+        const size_t q = (size_t)evalIdx * numTiles + t;
+        r.lnL        += __ldcg (&ctx.tilePartial[q].x);
+        r.unobserved += __ldcg (&ctx.tilePartial[q].y);       // dead, and not loaded, where the caller ignores it
+        r.abort      |= __ldcg (&ctx.tileAbort[q]);
+        }
+    ctx.ticket[evalIdx] = 0u;
+    return r;
+}
 
 static inline size_t mb200_align16 (size_t x) { return (x + 15) & ~(size_t)15; }

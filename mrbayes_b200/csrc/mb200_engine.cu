@@ -91,7 +91,7 @@ struct Instance
     size_t        eigInStride = 0;
     std::vector<cudaEvent_t> evEigIn;    // per slot: the staging area has been read
     uint64_t     *dInvMask = nullptr;
-    double       *dTilePartial = nullptr;
+    double2      *dTilePartial = nullptr;
     int          *dTileAbort = nullptr;
     unsigned int *dTicket = nullptr;
     bool          invMaskValid = false;
@@ -123,7 +123,6 @@ struct Instance
     StdCtx        sx;
     int          *dStdTab = nullptr;   // nStates | tiIndex | bsIndex, [3][C]
     int2         *dStdClasses = nullptr;
-    double       *dTilePartial2 = nullptr;
     std::vector<int> hNStates, hTiIndex, hBsIndex;
     std::vector<size_t> hClOff;        // ragged host layout: offset of pattern c inside a category's block
     bool          timing = false;      // bracket the fused kernel with events
@@ -550,7 +549,6 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
         d.pInvar = ev.p_invar;
         d.dOff = dblPos;
         dblPos += 2*K + nFreq + (ev.inline_eigen ? 2*S + S*S*S : 0);
-        d.fuseP = fused ? 1 : 0;
         d.eigen0 = (ev.matrix_update_count > 0) ? ev.matrix_updates[0].eigen : 0;
         d.nChunk = nChunkOf[e];
         d.chunkOff = extraPos;
@@ -1125,7 +1123,7 @@ void destroy (Instance *I)
     cudaFree (I->dTip8); cudaFree (I->dTip64); cudaFree (I->dTipPartAmbig); cudaFree (I->dSplit); cudaFree (I->dPartials); cudaFree (I->dMatrices);
     cudaFree (I->dScalers); cudaFree (I->dWeights); cudaFree (I->dEigen); cudaFree (I->dFactor); cudaFree (I->dInvMask);
     cudaFree (I->dTilePartial); cudaFree (I->dTileAbort); cudaFree (I->dTicket);
-    cudaFree (I->dStdTab); cudaFree (I->dStdClasses); cudaFree (I->dTilePartial2);
+    cudaFree (I->dStdTab); cudaFree (I->dStdClasses);
     cudaFree (I->dTcCounter); cudaFree (I->dTcFlags); cudaFree (I->dTcError);
     cudaFree (I->dEigIn); if (I->dEigVec != I->dFactor) cudaFree (I->dEigVec);
     cudaFree (I->dEigU); cudaFree (I->dEigLog); cudaFree (I->dEigRounds);
@@ -1277,17 +1275,15 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
         cudaMemsetAsync (I->dTcFlags, 0, nFlags * sizeof(int), I->stream);
         }
     ALLOC (I->dInvMask,  (size_t)C * sizeof(uint64_t));
-    ALLOC (I->dTilePartial, (size_t)I->maxEval * I->maxTiles * sizeof(double));
+    ALLOC (I->dTilePartial, (size_t)I->maxEval * I->maxTiles * sizeof(double2));
     ALLOC (I->dTileAbort,   (size_t)I->maxEval * I->maxTiles * sizeof(int));
     ALLOC (I->dTicket,      (size_t)I->maxEval * sizeof(unsigned int));
     if (I->std)
         {
         ALLOC (I->dStdTab,       (size_t)3 * C * sizeof(int));
         ALLOC (I->dStdClasses,   (size_t)MB200_STD_MAX_STATES * sizeof(int2));
-        ALLOC (I->dTilePartial2, (size_t)I->maxEval * I->maxTiles * 2 * sizeof(double));
         memset (&I->sx, 0, sizeof(I->sx));
         I->sx.lanes = stdLanes;
-        I->sx.tilePartial2 = I->dTilePartial2;
         }
 #undef ALLOC
     cudaMemsetAsync (I->dTip8, 0, (size_t)cfg->tip_count * C, I->stream);

@@ -36,7 +36,6 @@ struct StdCtx                       // variable-state tables of an instance, pas
     int         dummy;              // leading unobservable patterns
     int         uncompressed;       // sites the coding-bias correction applies to
     int         lanes;              // L: lanes per pattern
-    double     *tilePartial2;       // [maxEval][numTiles][2]: weighted log terms, unobserved probability
 };
 
 // ---------------------------------------------------------------------------------------
@@ -51,14 +50,7 @@ tiprobs_std_kernel (DevCtx ctx, StdCtx sx, const DevEval *__restrict__ evals, in
     __shared__ int sEvalIdx;
     const DevMat mu = mats[blockIdx.x];
     if (threadIdx.x == 0)
-        {
-        int e = 0;                                // the evaluation whose update list holds this matrix
-        while (e + 1 < nEval && (int) blockIdx.x >= evals[e + 1].matOff)
-            e++;
-        while (e > 0 && evals[e].nMat == 0)
-            e--;
-        sEvalIdx = e;
-        }
+        sEvalIdx = owning_eval (evals, nEval, blockIdx.x);
     __syncthreads ();
     const double *rates = dvals + evals[sEvalIdx].dOff;
     double length = mu.length;
@@ -118,7 +110,6 @@ eval_std_kernel (DevCtx ctx, StdCtx sx, const DevEval *__restrict__ evals, const
 {
     __shared__ double sSum[NT/32], sUn[NT/32];
     __shared__ int    sAb[NT/32];
-    __shared__ int    sLast;
     const int L = sx.lanes, TP = NT / L, K = ctx.K, C = ctx.C, Sp = ctx.Sp;
     const int p = threadIdx.x / L, k = threadIdx.x % L;
     const int c = blockIdx.x * TP + p;
@@ -255,33 +246,15 @@ eval_std_kernel (DevCtx ctx, StdCtx sx, const DevEval *__restrict__ evals, const
         double s = 0.0, u = 0.0; int a = 0;
         #pragma unroll
         for (int w = 0; w < NT/32; w++) { s += sSum[w]; u += sUn[w]; a |= sAb[w]; }
-        const size_t slot = (size_t)blockIdx.y * ctx.numTiles + blockIdx.x;
-        sx.tilePartial2[2*slot] = s; sx.tilePartial2[2*slot + 1] = u;
-        ctx.tileAbort[slot] = a;
-        __threadfence ();
-        const unsigned int t = atomicAdd (&ctx.ticket[blockIdx.y], 1u);
-        sLast = (t == (unsigned int) ctx.numTiles - 1u);
-        if (sLast)
+        if (tile_arrive (ctx, blockIdx.y, ctx.numTiles, blockIdx.x, make_double2 (s, u), a))
             {
-            __threadfence ();
-            double tot = 0.0, un = 0.0; int ab = 0;
-            for (int tIdx = 0; tIdx < ctx.numTiles; tIdx++)
-                {
-                const size_t q = (size_t)blockIdx.y * ctx.numTiles + tIdx;
-                tot += __ldcg (&sx.tilePartial2[2*q]);
-                un  += __ldcg (&sx.tilePartial2[2*q + 1]);
-                ab  |= __ldcg (&ctx.tileAbort[q]);
-                }
+            const TileSum ts = tile_sum_ltr (ctx, blockIdx.y, ctx.numTiles);
             // correct for absent characters (src/likelihood.c:7417-7423, 7537)
-            double pObserved = 1.0 - un;
+            double pObserved = 1.0 - ts.unobserved;
             if (pObserved < MB200_LIKE_EPSILON)
                 pObserved = MB200_LIKE_EPSILON;
-            tot -= log (pObserved) * (double) sx.uncompressed;
-            const double lnL = ab ? -DBL_MAX : tot;
-            int4 pkt;
-            pkt.x = __double2loint (lnL); pkt.y = __double2hiint (lnL); pkt.z = ab ? 1 : 0; pkt.w = seq;
-            *reinterpret_cast<int4 *>(&out[blockIdx.y]) = pkt;
-            ctx.ticket[blockIdx.y] = 0u;
+            const double tot = ts.lnL - log (pObserved) * (double) sx.uncompressed;
+            dev_result_write (&out[blockIdx.y], ts.abort ? -DBL_MAX : tot, ts.abort ? 1 : 0, seq);
             }
         }
 }

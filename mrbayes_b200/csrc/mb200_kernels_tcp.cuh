@@ -583,25 +583,11 @@ eval_tcp_kernel (DevCtx ctx, TcQueue Q, int NS, const DevEval *__restrict__ eval
                 {
                 const double s = qSum[grp][0] + qSum[grp][1] + qSum[grp][2] + qSum[grp][3];
                 const int    a = qAb[grp][0] | qAb[grp][1] | qAb[grp][2] | qAb[grp][3];
-                ctx.tilePartial[(size_t)it.e * numTiles + it.t] = s;
-                ctx.tileAbort  [(size_t)it.e * numTiles + it.t] = a;
-                __threadfence ();
-                const unsigned int tk = atomicAdd (&ctx.ticket[it.e], 1u);
-                if (tk == (unsigned int) numTiles - 1u)
+                if (tile_arrive (ctx, it.e, numTiles, it.t, make_double2 (s, 0.0), a))
                     {
-                    __threadfence ();
-                    double tot = 0.0; int ab = 0;
-                    for (int tIdx = 0; tIdx < numTiles; tIdx++)
-                        {
-                        tot += __ldcg (&ctx.tilePartial[(size_t)it.e * numTiles + tIdx]);
-                        ab  |= __ldcg (&ctx.tileAbort  [(size_t)it.e * numTiles + tIdx]);
-                        }
-                    if (*((volatile int *) Q.error)) ab = 1;
-                    const double lnL = ab ? -DBL_MAX : tot;
-                    int4 pkt;
-                    pkt.x = __double2loint (lnL); pkt.y = __double2hiint (lnL); pkt.z = ab ? 1 : 0; pkt.w = seq;
-                    *reinterpret_cast<int4 *>(&out[it.e]) = pkt;
-                    ctx.ticket[it.e] = 0u;
+                    const TileSum ts = tile_sum_ltr (ctx, it.e, numTiles);
+                    const int ab = ts.abort | *((volatile int *) Q.error);
+                    dev_result_write (&out[it.e], ab ? -DBL_MAX : ts.lnL, ab ? 1 : 0, seq);
                     }
                 }
             tcp_bar_group (grp);                               // qSum / qAb free for the group's next closing item
