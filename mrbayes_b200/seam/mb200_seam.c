@@ -25,6 +25,13 @@
  * working unmodified; the engine is addressed purely by the indices valid at
  * call time.  One LogLike call == one mb200_evaluate == one fused GPU pass.
  *
+ * Four ways in, one evaluation record (mb200_evaluation) and one dispatch (SeamRootAndLaunch) behind them: the
+ * mbbeagle.h entry points above; MB200LaunchLogLikeForDivision / MB200LogLike (replacements for
+ * LaunchLogLikeForDivision and the division loop of LogLike: all divisions of a chain in flight together); MB200Batch*
+ * (chain-batched generations: all local chains of a generation in one engine call); TiProbs_B200 ... Likelihood_B200
+ * (node-granular function-pointer forms driven by the reference's own LaunchLogLikeForDivision loop).  Besides them
+ * the host readers installed by MB200InstallReaders.
+ *
  * No reference source text is copied: only the public structs and function
  * prototypes of the reference headers are used.
  */
@@ -49,6 +56,14 @@ int SetProteinQMatrix (MrBFlt **a, int n, int whichChain, int division, MrBFlt r
 
 #define SEAM_MAX_DIVISIONS 512
 
+/* per local chain: dynamic rescaling (MB200_RESCALE=dynamic), the rescale frequency and the run of clean evaluations;
+   how many nodes the retry flipped beyond the move's own (SeamDivision.extraFlip); state[] when the chain was queued */
+typedef struct { int dynFreq, dynRun, nExtraFlip, queuedState; } SeamChain;
+
+/* one set of scratch indices of a division, what ModelInfo's *ScratchIndex fields and unscaledNodesScratch hold:
+   [node] conditional likelihoods, P(t), node scalers, unscaled nodes; site scalers; eigensystem */
+typedef struct { int *cl, *ti, *ns, *un; int site, cijk; } SeamScratch;
+
 typedef struct
     {
     int                  instance;          /* engine instance, -1 = none            */
@@ -68,17 +83,21 @@ typedef struct
     mb200_matrix_update *matsArena;         /* [nSlots][capMats] */
     double              *eigArena;          /* [nSlots][72]      */
     mb200_evaluation    *qEv;               /* [nSlots] evaluations queued this generation */
-    int                 *qChain, *qStatus;  /* [nSlots] */
-    double              *qLnL;              /* [nSlots] */
-    int                  qRc, qLaunched;
+    int                 *qChain;            /* [nSlots] ... and their chains */
+    int                  qLaunched;
+    /* results of the evaluations started last (SeamStart / SeamFinish): the queue's, or in [0] a deferred single evaluation's */
+    double              *qLnL;              /* [nSlots], the tail of eigArena's block */
+    int                 *qStatus;           /* [nSlots], the head of the block that also holds qChain and extraFlip */
+    int                  qRc, inFlight;     /* inFlight: started with evaluate_begin, evaluate_end fetches the results */
+    SeamChain           *chains;            /* [nSlots] */
+    int                 *extraFlip;         /* [nSlots][capOps] nodes the retry flipped beyond the move's own */
     /* per-chain scratch sets: the reference keeps ONE scratch slot per node, shared by all chains
        (src/mcmc.c:5940-5949), which is fine while a chain is accepted or rejected before the next one is
        touched; with the accept step deferred every chain needs its own.  Chain 0 keeps the reference's. */
     int                  nScratchChains, scratchNodes;
-    int                **scrCl, **scrTi, **scrNs, **scrUn;  /* [chain][node]; [0] unused */
-    int                 *scrSite, *scrCijk;                  /* [chain] */
-    int                 *origCl, *origTi, *origNs, *origUn; /* the reference's arrays while a chain's set is installed */
-    int                  origSite, origCijk, installed;     /* installed: chain whose set is in place, or -1 */
+    SeamScratch         *scr;               /* [chain]; [0] unused; the four arrays of a chain are one block (cl) */
+    SeamScratch          orig;              /* the reference's set while a chain's is installed */
+    int                  installed;         /* chain whose set is in place, or -1 */
     int                  extraCl, extraTi, extraNs, extraEig;  /* buffers beyond the reference's own counts */
     MrBFlt             **extraCijks;        /* host eigensystem blocks appended to m->cijks for the extra slots */
     /* host readers (MB200InstallReaders): the reference's own function pointers, what the host arrays currently mirror,
@@ -93,17 +112,11 @@ typedef struct
     int                  nHostExtra;
     int                  stdHostP;          /* STANDARD division whose P(t) the reference's TiProbs_Std builds on the host */
     int                  hostPFailed;       /* ... and one of this evaluation's matrices could not be built or shipped */
-    /* dynamic rescaling (MB200_RESCALE=dynamic): per chain, the rescale frequency and the run of clean evaluations */
-    int                 *dynFreq, *dynRun;
-    int                 *extraFlip, *nExtraFlip, *queuedState;  /* [chain][capOps] nodes the retry flipped beyond the move's own;
-                                                                   [chain] how many; [chain] state[] when the chain was queued */
-    int                  guard;             /* the evaluation being assembled was built with a rescale frequency > 1 */
+    int                  guard;             /* dynamic rescaling: the evaluation being assembled was built with a rescale frequency > 1 */
     long long            dynRetries;
     long long            clUpdates;         /* node*pattern*rate updates issued      */
     int                  pending;           /* launched by a deferred evaluation, result not yet collected */
     int                  recording, recChain, recState;   /* function-pointer forms: evaluation being recorded */
-    double               syncValue;         /* backend without begin/end: the result, kept until collected */
-    int                  syncStatus, syncRc;
     } SeamDivision;
 
 static SeamDivision seamDiv[SEAM_MAX_DIVISIONS];
@@ -112,6 +125,13 @@ static int          seamInitialized = NO;
    the device has never seen uploads it first: chains whose first evaluation ran on the
    reference's own path, or an instance that was re-created. */
 static unsigned char seamCijkSeen[SEAM_MAX_DIVISIONS][(2 * MAX_CHAINS + 8) / 8 + 1];
+
+/* bit sets (seamCijkSeen, the per-chain division flags seamFlag*) */
+static inline int  SeamBitGet (const unsigned char *set, int i)         { return (set[i >> 3] >> (i & 7)) & 1; }
+static inline void SeamBitAssign (unsigned char *set, int i, int on)
+{
+    set[i >> 3] = (unsigned char)((set[i >> 3] & ~(1 << (i & 7))) | ((on ? 1 : 0) << (i & 7)));
+}
 
 /* ---- backend indirection: lets the oracle harness record or shadow every call ---- */
 static int be_create (const mb200_instance_config *c, int *i)          { return mb200_create_instance (c, i); }
@@ -129,10 +149,15 @@ static int be_gets (int i, int s, float *o)                            { return 
 static int be_setm (int i, int m, const float *in)                     { return mb200_set_transition_matrix (i, m, in); }
 static int be_rates (int i, int e, int l, const double *q, const double *f) { return mb200_set_rate_matrices (i, e, l, q, f); }
 
-static MB200SeamBackend seamBackend = { be_create, be_finalize, be_tips, be_weights, be_cijk, be_eval, be_begin, be_end, be_pstates, be_getp, be_getm, be_gets, be_setm, be_rates };
-static int seamDeferred = NO;   /* YES: TreeLikelihood_Beagle only launches; SeamCollect fetches the result */
+static const MB200SeamBackend seamEngine = { be_create, be_finalize, be_tips, be_weights, be_cijk, be_eval, be_begin, be_end, be_pstates, be_getp, be_getm, be_gets, be_setm, be_rates };
+static MB200SeamBackend        seamCustomBackend;           /* the table MB200SeamSetBackend was given */
+static const MB200SeamBackend *seamBackend = &seamEngine;
+/* what SeamRootAndLaunch does with the evaluation it has assembled: evaluate it and hand the result back; start it and
+   let SeamCollect fetch the result (MB200LogLike, LaunchBEAGLELogLikeMultiPartition); keep it in the division's queue
+   until MB200BatchFlush (MB200BatchQueueLogLike) */
+enum { SEAM_RUN_NOW, SEAM_RUN_DEFERRED, SEAM_RUN_QUEUED };
+static int seamRun = SEAM_RUN_NOW;
 static int seamBatchWanted = NO;    /* MB200BatchEnable: instances are created with per-chain scratch buffers */
-static int seamBatchQueue = NO;     /* YES while MB200BatchQueueLogLike assembles: evaluations are queued, not launched */
 static void SeamScratchCounts (ModelInfo *m, int *nCl, int *nTi, int *nNs);
 static int  SeamReadersWanted (ModelInfo *m);
 static void SeamDropDivision (int division);
@@ -140,12 +165,12 @@ static void SeamDropDivision (int division);
 void MB200SeamSetBackend (const MB200SeamBackend *backend)
 {
     if (backend == NULL)
-        {
-        MB200SeamBackend def = { be_create, be_finalize, be_tips, be_weights, be_cijk, be_eval, be_begin, be_end, be_pstates, be_getp, be_getm, be_gets, be_setm, be_rates };
-        seamBackend = def;
-        }
+        seamBackend = &seamEngine;
     else
-        seamBackend = *backend;
+        {
+        seamCustomBackend = *backend;
+        seamBackend = &seamCustomBackend;
+        }
 }
 
 static void SeamInit (void)
@@ -162,7 +187,6 @@ static void SeamInit (void)
     seamInitialized = YES;
 }
 
-/* dynamic rescaling: evaluations repeated with every node rescaled after an underflow (all divisions) */
 /* host time spent on eigensystems (UpDateCijk: rate matrix, GetEigens, CalcCijk) and on shipping them to the engine */
 static double    seamSecCijk = 0.0, seamSecCijkUpload = 0.0;
 static long long seamCijkUpdates = 0;
@@ -364,7 +388,7 @@ static int SeamStdDivision (ModelInfo *m)
         }
     if (freqLen > MB200_MAX_STATES)
         return NO;
-    if (SeamStdHostMatrices (m) == YES && seamBackend.set_transition_matrix == NULL)
+    if (SeamStdHostMatrices (m) == YES && seamBackend->set_transition_matrix == NULL)
         return NO;
     return YES;
 }
@@ -420,11 +444,11 @@ int MB200SeamDivisionSupported (ModelInfo *m)
     if (m->nParsIntsPerSite != 1)
         return NO;
     if ((m->printPosSel == YES || m->printSiteOmegas == YES) &&
-        (seamBackend.get_partials == NULL || SeamOmegaCategories (m) == NO || getenv ("MB200_NO_READERS") != NULL))
+        (seamBackend->get_partials == NULL || SeamOmegaCategories (m) == NO || getenv ("MB200_NO_READERS") != NULL))
         return NO;                              /* PosSelProbs / SiteOmegas read the root's conditional likelihoods on the host
                                                    (src/mcmc.c:5761-5772, 12627, 12664): MB200InstallReaders wraps them too */
     if (SeamReadersWanted (m) == YES &&
-        (seamBackend.get_partials == NULL || seamBackend.get_transition_matrix == NULL || seamBackend.get_scalers == NULL ||
+        (seamBackend->get_partials == NULL || seamBackend->get_transition_matrix == NULL || seamBackend->get_scalers == NULL ||
          m->numOmegaCats != 1 || getenv ("MB200_NO_READERS") != NULL))
         return NO;                              /* ancestral states / site rates without a read-back path */
     return YES;
@@ -539,38 +563,39 @@ void MB200SeamDivisionConfig (ModelInfo *m, int division, mb200_instance_config 
  * installing a chain's own scratch arrays in ModelInfo before its proposal, evaluation or ResetFlips and
  * putting the reference's arrays back afterwards gives every chain a private double buffer without touching
  * any of the reference's code. */
+/* puts *s into ModelInfo and returns the set that was there */
+static SeamScratch SeamSwapScratch (ModelInfo *m, const SeamScratch *s)
+{
+    const SeamScratch was = { m->condLikeScratchIndex, m->tiProbsScratchIndex, m->nodeScalerScratchIndex, m->unscaledNodesScratch,
+                              m->siteScalerScratchIndex, m->cijkScratchIndex };
+    m->condLikeScratchIndex   = s->cl;
+    m->tiProbsScratchIndex    = s->ti;
+    m->nodeScalerScratchIndex = s->ns;
+    m->unscaledNodesScratch   = s->un;
+    m->siteScalerScratchIndex = s->site;
+    m->cijkScratchIndex       = (s->cijk >= 0) ? s->cijk : was.cijk;    /* no cijk slot of its own: the one in place stays */
+    return was;
+}
+
 static void SeamInstallScratch (ModelInfo *m, SeamDivision *sd, int chain)
 {
     if (chain < 1 || chain >= sd->nScratchChains || sd->installed >= 0)
         return;
-    sd->origCl = m->condLikeScratchIndex;    sd->origTi = m->tiProbsScratchIndex;
-    sd->origNs = m->nodeScalerScratchIndex;  sd->origUn = m->unscaledNodesScratch;
-    sd->origSite = m->siteScalerScratchIndex; sd->origCijk = m->cijkScratchIndex;
-    m->condLikeScratchIndex   = sd->scrCl[chain];
-    m->tiProbsScratchIndex    = sd->scrTi[chain];
-    m->nodeScalerScratchIndex = sd->scrNs[chain];
-    m->unscaledNodesScratch   = sd->scrUn[chain];
-    m->siteScalerScratchIndex = sd->scrSite[chain];
-    if (sd->scrCijk[chain] >= 0)
-        m->cijkScratchIndex   = sd->scrCijk[chain];
+    sd->orig = SeamSwapScratch (m, &sd->scr[chain]);
     sd->installed = chain;
 }
 
 static void SeamRestoreScratch (ModelInfo *m, SeamDivision *sd)
 {
-    int chain = sd->installed;
+    SeamScratch *mine, was;
 
-    if (chain < 0)
+    if (sd->installed < 0)
         return;
-    sd->scrSite[chain] = m->siteScalerScratchIndex;      /* scalars travel by value; the arrays were flipped in place */
-    if (sd->scrCijk[chain] >= 0)
-        sd->scrCijk[chain] = m->cijkScratchIndex;
-    m->condLikeScratchIndex   = sd->origCl;
-    m->tiProbsScratchIndex    = sd->origTi;
-    m->nodeScalerScratchIndex = sd->origNs;
-    m->unscaledNodesScratch   = sd->origUn;
-    m->siteScalerScratchIndex = sd->origSite;
-    m->cijkScratchIndex       = sd->origCijk;
+    mine = &sd->scr[sd->installed];
+    was = SeamSwapScratch (m, &sd->orig);
+    mine->site = was.site;              /* scalars travel by value; the arrays were flipped in place */
+    if (mine->cijk >= 0)
+        mine->cijk = was.cijk;
     sd->installed = -1;
 }
 
@@ -584,14 +609,9 @@ static int SeamBuildScratchSets (ModelInfo *m, SeamDivision *sd)
     nNodes = t->nNodes;
     sd->scratchNodes = nNodes;
     sd->nScratchChains = n;
-    sd->scrCl   = (int **) SafeCalloc ((size_t)n, sizeof(int *));
-    sd->scrTi   = (int **) SafeCalloc ((size_t)n, sizeof(int *));
-    sd->scrNs   = (int **) SafeCalloc ((size_t)n, sizeof(int *));
-    sd->scrUn   = (int **) SafeCalloc ((size_t)n, sizeof(int *));
-    sd->scrSite = (int *)  SafeCalloc ((size_t)n, sizeof(int));
-    sd->scrCijk = (int *)  SafeCalloc ((size_t)n, sizeof(int));
-    sd->extraCijks = (MrBFlt **) SafeCalloc ((size_t)n, sizeof(MrBFlt *));
-    if (!sd->scrCl || !sd->scrTi || !sd->scrNs || !sd->scrUn || !sd->scrSite || !sd->scrCijk || !sd->extraCijks)
+    sd->scr        = (SeamScratch *) SafeCalloc ((size_t)n, sizeof(SeamScratch));
+    sd->extraCijks = (MrBFlt **)     SafeCalloc ((size_t)n, sizeof(MrBFlt *));
+    if (!sd->scr || !sd->extraCijks)
         return (ERROR);
     nextCl  = m->numCondLikes;
     nextTi  = m->numTiProbs;
@@ -607,28 +627,29 @@ static int SeamBuildScratchSets (ModelInfo *m, SeamDivision *sd)
         }
     for (c=1; c<n; c++)
         {
-        sd->scrCl[c] = (int *) SafeMalloc ((size_t)nNodes * sizeof(int));
-        sd->scrTi[c] = (int *) SafeMalloc ((size_t)nNodes * sizeof(int));
-        sd->scrNs[c] = (int *) SafeMalloc ((size_t)nNodes * sizeof(int));
-        sd->scrUn[c] = (int *) SafeMalloc ((size_t)nNodes * sizeof(int));
-        if (!sd->scrCl[c] || !sd->scrTi[c] || !sd->scrNs[c] || !sd->scrUn[c])
+        SeamScratch *s = &sd->scr[c];
+        s->cl = (int *) SafeMalloc ((size_t)4 * nNodes * sizeof(int));
+        if (!s->cl)
             return (ERROR);
+        s->ti = s->cl + nNodes;
+        s->ns = s->ti + nNodes;
+        s->un = s->ns + nNodes;
         for (i=0; i<nNodes; i++)
             {
-            sd->scrCl[c][i] = (m->condLikeScratchIndex[i]   >= 0) ? nextCl++ : -1;
-            sd->scrTi[c][i] = (m->tiProbsScratchIndex[i]    >= 0) ? nextTi++ : -1;
-            sd->scrNs[c][i] = (m->nodeScalerScratchIndex[i] >= 0) ? nextNs++ : -1;
-            sd->scrUn[c][i] = m->unscaledNodesScratch[i];
+            s->cl[i] = (m->condLikeScratchIndex[i]   >= 0) ? nextCl++ : -1;
+            s->ti[i] = (m->tiProbsScratchIndex[i]    >= 0) ? nextTi++ : -1;
+            s->ns[i] = (m->nodeScalerScratchIndex[i] >= 0) ? nextNs++ : -1;
+            s->un[i] = m->unscaledNodesScratch[i];
             }
-        sd->scrSite[c] = nextNs++;
-        sd->scrCijk[c] = -1;
+        s->site = nextNs++;
+        s->cijk = -1;
         if (m->cijks != NULL && m->nCijkParts > 0 && m->cijkLength > 0)
             {
             sd->extraCijks[c] = (MrBFlt *) SafeMalloc ((size_t)m->cijkLength * sizeof(MrBFlt));
             if (!sd->extraCijks[c])
                 return (ERROR);
             m->cijks[nextEig] = sd->extraCijks[c];
-            sd->scrCijk[c] = nextEig++;
+            s->cijk = nextEig++;
             }
         }
     return (NO_ERROR);
@@ -643,24 +664,20 @@ static void SeamDropDivision (int division)
     if (sd->installed >= 0)
         SeamRestoreScratch (&modelSettings[division], sd);
     if (sd->instance >= 0)
-        seamBackend.finalize_instance (sd->instance);
+        seamBackend->finalize_instance (sd->instance);
     free (sd->opsArena);
     free (sd->matsArena);
-    free (sd->eigArena);
-    free (sd->qEv); free (sd->qChain); free (sd->qStatus); free (sd->qLnL);
+    free (sd->eigArena); free (sd->qStatus);    /* with qLnL; with qChain and extraFlip */
+    free (sd->qEv); free (sd->chains);
     for (c=0; c<sd->nHostExtra; c++)
         free (sd->hostExtra[c]);
     free (sd->hostExtra);
-    free (sd->dynFreq); free (sd->dynRun); free (sd->extraFlip); free (sd->nExtraFlip); free (sd->queuedState);
     for (c=1; c<sd->nScratchChains; c++)
         {
-        if (sd->scrCl) free (sd->scrCl[c]);
-        if (sd->scrTi) free (sd->scrTi[c]);
-        if (sd->scrNs) free (sd->scrNs[c]);
-        if (sd->scrUn) free (sd->scrUn[c]);
+        if (sd->scr) free (sd->scr[c].cl);
         if (sd->extraCijks) free (sd->extraCijks[c]);
         }
-    free (sd->scrCl); free (sd->scrTi); free (sd->scrNs); free (sd->scrUn); free (sd->scrSite); free (sd->scrCijk);
+    free (sd->scr);
     free (sd->extraCijks);
     {
     /* the reference's reader pointers outlive the instance (the wrappers stay installed in ModelInfo) */
@@ -686,6 +703,19 @@ static void SeamSelectSlot (SeamDivision *sd, int q)
     sd->eigenBlock = sd->eigArena  + (size_t)q * 72;
 }
 
+/* Does the cached instance of a division still fit the model?  Two tests: this one runs for every evaluation, so it
+   compares pointers and counts only -- another mcmc command in the same session (new model, character set or chain count)
+   reallocates the reference's data and changes these; InitBeagleInstance, once per run and whenever this test answers YES,
+   compares the whole configuration and a checksum of the tip data before it keeps or rebuilds the instance. */
+static int SeamInstanceStale (ModelInfo *m, SeamDivision *sd)
+{
+    return (sd->parsPtr != (const void *) m->parsSets || sd->weightPtr != (const void *) numSitesOfPat ||
+        sd->cfg.pattern_count != m->numChars || sd->cfg.category_count != SeamCategories (m) ||
+        sd->cfg.partials_count != m->numCondLikes + sd->extraCl || sd->cfg.matrix_count != m->numTiProbs + sd->extraTi ||
+        sd->cfg.scaler_count != m->numScalers + sd->extraNs || (m->dataType != STANDARD && sd->cfg.state_count != m->numModelStates) ||
+        sd->cfg.weight_rows != chainParams.numChains || sd->cfg.eigen_count != numLocalChains + 1 + sd->extraEig) ? YES : NO;
+}
+
 /* ---- InitBeagleInstance (src/mbbeagle.c:60): allocate device buffers, load tips ---- */
 int InitBeagleInstance (ModelInfo *m, int division)
 {
@@ -695,9 +725,10 @@ int InitBeagleInstance (ModelInfo *m, int division)
     SeamDivision           *sd;
     mb200_operation        *ops = NULL;
     mb200_matrix_update    *mats = NULL;
-    double                 *eigs = NULL, *qLnL = NULL;
     mb200_evaluation       *qEv = NULL;
-    int                    *qChain = NULL, *qStatus = NULL, *dynF = NULL, *dynR = NULL, *xFlip = NULL, *nXFlip = NULL, *qState = NULL;
+    double                 *dbl = NULL;     /* eigArena [nSlots][72], qLnL [nSlots] */
+    int                    *ints = NULL;    /* qStatus [nSlots], qChain [nSlots], extraFlip [nSlots][capOps] */
+    SeamChain              *chains = NULL;
 
     SeamInit ();
     if (division < 0 || division >= SEAM_MAX_DIVISIONS)
@@ -725,23 +756,17 @@ int InitBeagleInstance (ModelInfo *m, int division)
     nSlots = (numLocalChains > 0) ? numLocalChains : 1;
     ops   = (mb200_operation *)     SafeCalloc ((size_t)nSlots * m->numCondLikes, sizeof(mb200_operation));
     mats  = (mb200_matrix_update *) SafeCalloc ((size_t)nSlots * m->numTiProbs,  sizeof(mb200_matrix_update));
-    eigs  = (double *)              SafeCalloc ((size_t)nSlots * 72, sizeof(double));
     qEv   = (mb200_evaluation *)    SafeCalloc ((size_t)nSlots, sizeof(mb200_evaluation));
-    qChain  = (int *)               SafeCalloc ((size_t)nSlots, sizeof(int));
-    qStatus = (int *)               SafeCalloc ((size_t)nSlots, sizeof(int));
-    qLnL  = (double *)              SafeCalloc ((size_t)nSlots, sizeof(double));
-    dynF  = (int *)                 SafeCalloc ((size_t)nSlots, sizeof(int));
-    dynR  = (int *)                 SafeCalloc ((size_t)nSlots, sizeof(int));
-    xFlip = (int *)                 SafeCalloc ((size_t)nSlots * m->numCondLikes, sizeof(int));
-    nXFlip = (int *)                SafeCalloc ((size_t)nSlots, sizeof(int));
-    qState = (int *)                SafeCalloc ((size_t)nSlots, sizeof(int));
+    dbl   = (double *)              SafeCalloc ((size_t)nSlots * (72 + 1), sizeof(double));
+    ints  = (int *)                 SafeCalloc ((size_t)nSlots * (2 + m->numCondLikes), sizeof(int));
+    chains = (SeamChain *)          SafeCalloc ((size_t)nSlots, sizeof(SeamChain));
     masks = (uint64_t *)            SafeMalloc ((size_t)m->numChars * sizeof(uint64_t));
-    if (!ops || !mats || !eigs || !qEv || !qChain || !qStatus || !qLnL || !dynF || !dynR || !xFlip || !nXFlip || !qState || !masks)
+    if (!ops || !mats || !qEv || !dbl || !ints || !chains || !masks)
         goto fail;
     for (i=0; i<nSlots; i++)
-        dynF[i] = 1;
+        chains[i].dynFreq = 1;
 
-    rc = seamBackend.create_instance (&cfg, &inst);
+    rc = seamBackend->create_instance (&cfg, &inst);
     if (rc != MB200_SUCCESS)
         {
         MrBayesPrint ("%s   H100 engine: cannot create instance for division %d (%s)\n", spacer, division+1, mb200_error_string (rc));
@@ -751,8 +776,8 @@ int InitBeagleInstance (ModelInfo *m, int division)
 
     if (m->dataType == STANDARD)
         {
-        if (seamBackend.set_pattern_states == NULL ||
-            seamBackend.set_pattern_states (inst, m->nStates, m->tiIndex, m->bsIndex, m->tiProbLength,
+        if (seamBackend->set_pattern_states == NULL ||
+            seamBackend->set_pattern_states (inst, m->nStates, m->tiIndex, m->bsIndex, m->tiProbLength,
                                             m->numDummyChars, m->numUncompressedChars) != MB200_SUCCESS)
             goto fail;
         }
@@ -773,14 +798,14 @@ int InitBeagleInstance (ModelInfo *m, int division)
             if (m->dataType == STANDARD)
                 masks[c] = obs;
             }
-        if (seamBackend.set_tip_states (inst, i, masks) != MB200_SUCCESS)
+        if (seamBackend->set_tip_states (inst, i, masks) != MB200_SUCCESS)
             goto fail;
         }
 
     /* pattern weights, one row per heat-ordered chain id (src/likelihood.c:5830) */
     for (i=0; i<chainParams.numChains; i++)
         {
-        if (seamBackend.set_pattern_weights (inst, i, numSitesOfPat + i*numCompressedChars + m->compCharStart) != MB200_SUCCESS)
+        if (seamBackend->set_pattern_weights (inst, i, numSitesOfPat + i*numCompressedChars + m->compCharStart) != MB200_SUCCESS)
             goto fail;
         }
     free (masks);
@@ -793,9 +818,9 @@ int InitBeagleInstance (ModelInfo *m, int division)
     sd->capOps   = m->numCondLikes;
     sd->capMats  = m->numTiProbs;
     sd->nSlots   = nSlots;
-    sd->opsArena = ops;   sd->matsArena = mats;  sd->eigArena = eigs;
-    sd->qEv = qEv; sd->qChain = qChain; sd->qStatus = qStatus; sd->qLnL = qLnL;
-    sd->dynFreq = dynF; sd->dynRun = dynR; sd->extraFlip = xFlip; sd->nExtraFlip = nXFlip; sd->queuedState = qState;
+    sd->opsArena = ops;   sd->matsArena = mats;  sd->qEv = qEv;  sd->chains = chains;
+    sd->eigArena = dbl;   sd->qLnL = dbl + (size_t)nSlots * 72;
+    sd->qStatus  = ints;  sd->qChain = ints + nSlots;  sd->extraFlip = ints + 2 * nSlots;
     sd->nQueued  = 0;
     SeamSelectSlot (sd, 0);
     memset (seamCijkSeen[division], 0, sizeof(seamCijkSeen[division]));
@@ -818,10 +843,8 @@ int InitBeagleInstance (ModelInfo *m, int division)
 
 fail:
     if (inst >= 0)
-        seamBackend.finalize_instance (inst);
-    free (ops);
-    free (mats);
-    free (eigs); free (qEv); free (qChain); free (qStatus); free (qLnL); free (dynF); free (dynR); free (xFlip); free (nXFlip); free (qState);
+        seamBackend->finalize_instance (inst);
+    free (ops); free (mats); free (qEv); free (dbl); free (ints); free (chains);
     free (masks);
     sd->instance = -1;
     return (ERROR);
@@ -858,25 +881,41 @@ static MrBFlt SeamBranchLength (ModelInfo *m, TreeNode *p, int chain)
 
 static int SeamHostBuffersFor (ModelInfo *m, SeamDivision *sd);
 
-static void SeamQueueMatrix (SeamDivision *sd, ModelInfo *m, TreeNode *p, int chain)
+/* this move cannot be evaluated: the signalling of Likelihood_* (src/likelihood.c:5857-5859); returns ERROR */
+static int SeamFailMove (MrBFlt *lnL)
 {
+    (*lnL) = MRBFLT_NEG_MAX;
+    abortMove = YES;
+    return (ERROR);
+}
+
+/* P(t) of the branch above p (its slot is flipped already): one more matrix-update record of the evaluation being
+   assembled -- or, in a stdHostP division, the matrix itself: the reference's TiProbs_Std fills the slot's host array and
+   the engine gets a copy */
+static int SeamMatrixRecord (ModelInfo *m, SeamDivision *sd, TreeNode *p, int chain)
+{
+    const int            idx = m->tiProbsIndex[chain][p->index];
     mb200_matrix_update *u;
 
-    FlipTiProbsSpace (m, chain, p->index);
     if (sd->stdHostP == YES)
         {
-        /* the reference's TiProbs_Std fills the slot's host array; the engine gets a copy.  (A chain-batched run gave the
-           chains slots beyond the reference's own table: SeamHostBuffersFor appends host arrays for them.) */
-        const int division = (int)(m - modelSettings), idx = m->tiProbsIndex[chain][p->index];
-        if (SeamHostBuffersFor (m, sd) == ERROR || TiProbs_Std (p, division, chain) == ERROR ||
-            seamBackend.set_transition_matrix (sd->instance, idx, m->tiProbs[idx]) != MB200_SUCCESS)
-            sd->hostPFailed = YES;
-        return;
+        return (TiProbs_Std (p, (int)(m - modelSettings), chain) == ERROR ||
+                seamBackend->set_transition_matrix (sd->instance, idx, m->tiProbs[idx]) != MB200_SUCCESS) ? ERROR : NO_ERROR;
         }
     u = &sd->mats[sd->ev.matrix_update_count++];
-    u->matrix = m->tiProbsIndex[chain][p->index];
+    u->matrix = idx;
     u->eigen  = (sd->inlineEigen == YES) ? MB200_EIGEN_INLINE : (m->dataType == STANDARD) ? MB200_NONE : m->cijkIndex[chain];
     u->length = SeamBranchLength (m, p, chain);
+    return (NO_ERROR);
+}
+
+static void SeamQueueMatrix (SeamDivision *sd, ModelInfo *m, TreeNode *p, int chain)
+{
+    FlipTiProbsSpace (m, chain, p->index);
+    /* (a chain-batched run gave the chains slots beyond the reference's own table: SeamHostBuffersFor appends host
+       arrays for them before TiProbs_Std writes one) */
+    if ((sd->stdHostP == YES && SeamHostBuffersFor (m, sd) == ERROR) || SeamMatrixRecord (m, sd, p, chain) == ERROR)
+        sd->hostPFailed = YES;
 }
 
 /* rate multipliers of TiProbs_Gen (src/likelihood.c:9432-9464): r_k = baseRate / (1 - pInvar) * catRate_k * corr */
@@ -956,6 +995,27 @@ int TreeTiProbs_Beagle (Tree *t, int division, int chain)
  *                   MB200BatchLeaveChain flips them back. */
 enum { SEAM_OPS_POLICY, SEAM_OPS_NONE, SEAM_OPS_ALL };
 
+/* destination, children and matrices of the update of node p, from the index tables as they stand (the caller has flipped
+   the node's conditional-likelihood space); isRoot: the three-neighbour update of CondLikeRoot_* */
+static void SeamOpRecord (ModelInfo *m, SeamDivision *sd, mb200_operation *op, TreeNode *p, int chain, int isRoot)
+{
+    op->dest    = m->condLikeIndex[chain][p->index];
+    op->child1  = m->condLikeIndex[chain][p->left->index];
+    op->matrix1 = m->tiProbsIndex [chain][p->left->index];
+    op->child2  = m->condLikeIndex[chain][p->right->index];
+    op->matrix2 = m->tiProbsIndex [chain][p->right->index];
+    op->child3  = (isRoot == YES) ? m->condLikeIndex[chain][p->anc->index] : MB200_NONE;
+    op->matrix3 = (isRoot == YES) ? m->tiProbsIndex [chain][p->index]      : MB200_NONE;
+    sd->clUpdates += (long long) m->numChars * SeamCategories (m);
+}
+
+/* scaler bookkeeping of src/likelihood.c:7938-7965: the node's old scaler leaves the site scalers when the node was
+   rescaled and the site scalers were copied, not reset; read BEFORE the node-scaler space is flipped */
+static int SeamScaleRemove (ModelInfo *m, TreeNode *p, int chain)
+{
+    return (m->unscaledNodes[chain][p->index] == 0 && m->upDateAll == NO) ? m->nodeScalerIndex[chain][p->index] : MB200_NONE;
+}
+
 static int SeamBuildOps (Tree *t, int division, int chain, int mode)
 {
     int                 i;
@@ -983,7 +1043,7 @@ static int SeamBuildOps (Tree *t, int division, int chain, int mode)
                 {
                 FlipCondLikeSpace (m, chain, p->index);
                 FlipNodeScalerSpace (m, chain, p->index);
-                sd->extraFlip[(size_t)chain * sd->capOps + sd->nExtraFlip[chain]++] = p->index;
+                sd->extraFlip[(size_t)chain * sd->capOps + sd->chains[chain].nExtraFlip++] = p->index;
                 }
             }
         else
@@ -992,31 +1052,13 @@ static int SeamBuildOps (Tree *t, int division, int chain, int mode)
                (src/likelihood.c:795-804) */
             FlipCondLikeSpace (m, chain, p->index);
             }
-        op->dest    = m->condLikeIndex[chain][p->index];
-        op->child1  = m->condLikeIndex[chain][p->left->index];
-        op->matrix1 = m->tiProbsIndex [chain][p->left->index];
-        op->child2  = m->condLikeIndex[chain][p->right->index];
-        op->matrix2 = m->tiProbsIndex [chain][p->right->index];
-        if (t->isRooted == NO && p->anc->anc == NULL)
-            {
-            op->child3  = m->condLikeIndex[chain][p->anc->index];
-            op->matrix3 = m->tiProbsIndex [chain][p->index];
-            }
-        else
-            {
-            op->child3  = MB200_NONE;
-            op->matrix3 = MB200_NONE;
-            }
+        SeamOpRecord (m, sd, op, p, chain, (t->isRooted == NO && p->anc->anc == NULL) ? YES : NO);
 
         if (mode == SEAM_OPS_ALL)
             op->scale_remove = MB200_NONE;              /* the site scalers start from zero */
         else
             {
-            /* scaler bookkeeping of src/likelihood.c:7938-7965 */
-            if (m->unscaledNodes[chain][p->index] == 0 && m->upDateAll == NO)
-                op->scale_remove = m->nodeScalerIndex[chain][p->index];
-            else
-                op->scale_remove = MB200_NONE;
+            op->scale_remove = SeamScaleRemove (m, p, chain);
             FlipNodeScalerSpace (m, chain, p->index);
             }
         m->unscaledNodes[chain][p->index] = 1 + m->unscaledNodes[chain][p->left->index]
@@ -1028,11 +1070,21 @@ static int SeamBuildOps (Tree *t, int division, int chain, int mode)
             }
         else
             op->scale_write = MB200_NONE;
-
-        sd->clUpdates += (long long) m->numChars * SeamCategories (m);
         }
 
     return (NO_ERROR);
+}
+
+/* the same with the chain's rescale frequency set to freq for the duration of the call: the reference's bookkeeping
+   field steers the policy (m->rescaleFreq is 1 in builds without BEAGLE, src/mcmc.c:6157-6164) */
+static void SeamBuildOpsAtFrequency (Tree *t, int division, int chain, int mode, int freq)
+{
+    ModelInfo *m = &modelSettings[division];
+    const int  savedFreq = m->rescaleFreq[chain];
+
+    m->rescaleFreq[chain] = freq;
+    SeamBuildOps (t, division, chain, mode);
+    m->rescaleFreq[chain] = savedFreq;
 }
 
 int TreeCondLikes_Beagle_Always_Rescale (Tree *t, int division, int chain)
@@ -1061,6 +1113,8 @@ int TreeCondLikes_Beagle_Rescale_All (Tree *t, int division, int chain)
  * which is why the default stays the reference's policy (bit-level parity). */
 static int seamDynMaxFreq = 8;      /* MB200_RESCALE_MAXFREQ */
 static int seamDynRun     = 200;    /* MB200_RESCALE_RUN: clean evaluations before the frequency grows */
+static int seamDynForceRetry = NO;  /* MB200_RESCALE_FORCE_RETRY=1 (tests): every evaluation takes the retry path */
+static int seamDynDebug   = NO;     /* MB200_RESCALE_DEBUG: one line on stderr per retry */
 
 static int SeamDynamicRescaling (void)
 {
@@ -1071,12 +1125,38 @@ static int SeamDynamicRescaling (void)
         mode = (s != NULL && strcmp (s, "dynamic") == 0) ? YES : NO;
         if ((s = getenv ("MB200_RESCALE_MAXFREQ")) != NULL && atoi (s) >= 1) seamDynMaxFreq = atoi (s);
         if ((s = getenv ("MB200_RESCALE_RUN")) != NULL && atoi (s) >= 1)     seamDynRun = atoi (s);
+        seamDynForceRetry = (getenv ("MB200_RESCALE_FORCE_RETRY") != NULL) ? YES : NO;
+        seamDynDebug      = (getenv ("MB200_RESCALE_DEBUG") != NULL) ? YES : NO;
         }
     return mode;
 }
 
+/* site scalers of the evaluation being assembled: the caller has flipped the site-scaler space; the reset or the copy
+   from the scratch slot (src/likelihood.c:7885-7889) happens on the device as part of the fused pass */
+static void SeamSiteScalers (ModelInfo *m, SeamDivision *sd, int chain)
+{
+    sd->ev.site_scaler_dst = m->siteScalerIndex[chain];
+    sd->ev.site_scaler_src = (m->upDateAll == YES) ? MB200_NONE : m->siteScalerScratchIndex;
+}
+
 static int SeamApplyResult (int division, int chain, int rc, double value, int status, MrBFlt *lnL);
 static int SeamRootAndLaunch (int division, int chain, int rootNode, MrBFlt *lnL, int whichSitePats);
+
+/* Start n evaluations of a division / finish them: return code in sd->qRc, results in sd->qLnL and sd->qStatus.  With
+   evaluate_begin / evaluate_end the device works between the two calls; a backend without the pair evaluates in SeamStart. */
+static void SeamStart (SeamDivision *sd, const mb200_evaluation *ev, int n)
+{
+    sd->inFlight = (seamBackend->evaluate_begin != NULL && seamBackend->evaluate_end != NULL) ? YES : NO;
+    sd->qRc = (sd->inFlight == YES) ? seamBackend->evaluate_begin (sd->instance, ev, n)
+                                    : seamBackend->evaluate (sd->instance, ev, n, sd->qLnL, sd->qStatus);
+}
+
+static void SeamFinish (SeamDivision *sd)
+{
+    if (sd->inFlight == YES && sd->qRc == MB200_SUCCESS)
+        sd->qRc = seamBackend->evaluate_end (sd->instance, sd->qLnL, sd->qStatus);
+    sd->inFlight = NO;
+}
 
 /* ---- TreeLikelihood_Beagle (src/mbbeagle.c:1117): root integration; launches ------- */
 int TreeLikelihood_Beagle (Tree *t, int division, int chain, MrBFlt *lnL, int whichSitePats)
@@ -1099,9 +1179,7 @@ static int SeamRootAndLaunch (int division, int chain, int rootNode, MrBFlt *lnL
     if (sd->hostPFailed == YES)
         {
         sd->hostPFailed = NO;
-        (*lnL) = MRBFLT_NEG_MAX;
-        abortMove = YES;
-        return (ERROR);
+        return SeamFailMove (lnL);
         }
     sd->evalStamp++;
     sd->ev.root_buffer = m->condLikeIndex[chain][rootNode];
@@ -1178,36 +1256,29 @@ static int SeamRootAndLaunch (int division, int chain, int rootNode, MrBFlt *lnL
             }
         }
 
-    if (seamBatchQueue == YES)
+    if (seamRun == SEAM_RUN_QUEUED)
         {
         /* chain-batched generation: the evaluation waits in the division's queue until MB200BatchFlush
            sends every chain's evaluation to the device in one call */
         int q = sd->nQueued;
         if (q >= sd->nSlots)
-            {
-            (*lnL) = MRBFLT_NEG_MAX;
-            abortMove = YES;
-            return (ERROR);
-            }
+            return SeamFailMove (lnL);
         sd->qEv[q]    = sd->ev;
         sd->qChain[q] = chain;
-        sd->queuedState[chain] = state[chain];
-        sd->nExtraFlip[chain]  = 0;
+        sd->chains[chain].queuedState = state[chain];
+        sd->chains[chain].nExtraFlip  = 0;
         sd->nQueued   = q + 1;
         SeamSelectSlot (sd, q + 1);
         return (NO_ERROR);
         }
-    if (seamDeferred == YES)
+    if (seamRun == SEAM_RUN_DEFERRED)
         {
-        /* partition-batched evaluation: launch only, MB200LogLike collects */
-        if (seamBackend.evaluate_begin != NULL && seamBackend.evaluate_end != NULL)
-            sd->syncRc = seamBackend.evaluate_begin (sd->instance, &sd->ev, 1);
-        else
-            sd->syncRc = seamBackend.evaluate (sd->instance, &sd->ev, 1, &sd->syncValue, &sd->syncStatus);
+        /* partition-batched evaluation: launch only, SeamCollect fetches the result */
+        SeamStart (sd, &sd->ev, 1);
         sd->pending = YES;
         return (NO_ERROR);
         }
-    rc = seamBackend.evaluate (sd->instance, &sd->ev, 1, &value, &status);
+    rc = seamBackend->evaluate (sd->instance, &sd->ev, 1, &value, &status);
     return SeamApplyResult (division, chain, rc, value, status, lnL);
 }
 
@@ -1218,8 +1289,7 @@ static int SeamRetryRescaleAll (int division, int chain, double *value, int *sta
     ModelInfo    *m  = &modelSettings[division];
     SeamDivision *sd = &seamDiv[division];
     Tree         *t  = GetTree (m->brlens, chain, state[chain]);
-    const mb200_evaluation failed = sd->ev;     /* root, weights row, rates, frequencies, pInvar: unchanged */
-    int           rc, savedFreq = m->rescaleFreq[chain];
+    int           rc;
 
     if (sd->nQueued > 0 && sd->qLaunched == YES)
         {
@@ -1233,16 +1303,14 @@ static int SeamRetryRescaleAll (int division, int chain, double *value, int *sta
         sd->ev = sd->qEv[q];
         SeamSelectSlot (sd, q);
         }
-    (void) failed;
-    m->rescaleFreq[chain] = 1;
-    SeamBuildOps (t, division, chain, SEAM_OPS_ALL);
-    m->rescaleFreq[chain] = savedFreq;
+    /* root, weights row, rates, frequencies, pInvar of the failed evaluation stay; the operations are built anew */
+    SeamBuildOpsAtFrequency (t, division, chain, SEAM_OPS_ALL, 1);
     sd->ev.matrix_update_count = 0;
     sd->ev.site_scaler_dst = m->siteScalerIndex[chain];
     sd->ev.site_scaler_src = MB200_NONE;
     sd->ev.flags &= ~MB200_FLAG_RANGE_GUARD;            /* every node rescaled: only a dead likelihood fails now */
     sd->dynRetries++;
-    rc = seamBackend.evaluate (sd->instance, &sd->ev, 1, value, status);
+    rc = seamBackend->evaluate (sd->instance, &sd->ev, 1, value, status);
     return (rc == MB200_SUCCESS) ? NO_ERROR : ERROR;
 }
 
@@ -1253,43 +1321,34 @@ static int SeamApplyResult (int division, int chain, int rc, double value, int s
 
     if (rc == MB200_SUCCESS && SeamDynamicRescaling () == YES && chain >= 0 && chain < sd->nSlots)
         {
-        static int forceRetry = -1;             /* MB200_RESCALE_FORCE_RETRY=1 (tests): every evaluation takes the retry path */
-        if (forceRetry < 0)
-            forceRetry = (getenv ("MB200_RESCALE_FORCE_RETRY") != NULL) ? YES : NO;
+        SeamChain *ch = &sd->chains[chain];
         if (sd->qLaunched == YES && sd->nQueued > 0 &&
-            ((status == MB200_EVAL_UNDERFLOW && sd->dynFreq[chain] > 1) || (forceRetry == YES && status == MB200_EVAL_OK)))
+            ((status == MB200_EVAL_UNDERFLOW && ch->dynFreq > 1) || (seamDynForceRetry == YES && status == MB200_EVAL_OK)))
             {
             const double failedValue = value;
-            const int    failedFreq = sd->dynFreq[chain];
-            sd->dynFreq[chain] = (sd->dynFreq[chain] + 1) / 2;
-            sd->dynRun[chain]  = 0;
+            const int    failedFreq = ch->dynFreq;
+            ch->dynFreq = (ch->dynFreq + 1) / 2;
+            ch->dynRun  = 0;
             if (SeamRetryRescaleAll (division, chain, &value, &status) == ERROR)
                 rc = MB200_ERROR_GENERAL;
-            if (getenv ("MB200_RESCALE_DEBUG") != NULL)
+            if (seamDynDebug == YES)
                 fprintf (stderr, "mb200 rescale retry: division %d chain %d freq %d: first attempt %.10g -> %.10g (status %d)\n",
                          division + 1, chain, failedFreq, failedValue, value, status);
             }
-        else if (status == MB200_EVAL_OK && modelSettings[division].numModelStates == 4 && ++sd->dynRun[chain] >= seamDynRun)
+        else if (status == MB200_EVAL_OK && modelSettings[division].numModelStates == 4 && ++ch->dynRun >= seamDynRun)
             {
-            sd->dynRun[chain] = 0;
-            if (sd->dynFreq[chain] < seamDynMaxFreq)
-                sd->dynFreq[chain]++;
+            ch->dynRun = 0;
+            if (ch->dynFreq < seamDynMaxFreq)
+                ch->dynFreq++;
             }
         }
     if (rc != MB200_SUCCESS)
         {
         MrBayesPrint ("%s   H100 engine: evaluation failed for division %d (%s)\n", spacer, division+1, mb200_error_string (rc));
-        (*lnL) = MRBFLT_NEG_MAX;
-        abortMove = YES;
-        return (ERROR);
+        return SeamFailMove (lnL);
         }
     if (status == MB200_EVAL_UNDERFLOW)
-        {
-        /* same signalling as Likelihood_* (src/likelihood.c:5857-5859) */
-        (*lnL) = MRBFLT_NEG_MAX;
-        abortMove = YES;
-        return (ERROR);
-        }
+        return SeamFailMove (lnL);
     (*lnL) = value;
     return (NO_ERROR);
 }
@@ -1299,25 +1358,19 @@ void LaunchBEAGLELogLikeForDivision (int chain, int d, ModelInfo *m, Tree *tree,
 {
     SeamDivision *sd = &seamDiv[d];
 
-    /* site scalers: flip, then reset or copy (src/likelihood.c:7885-7889); the copy
-       itself happens on the device as part of the fused pass */
+    /* site scalers: flip, then reset or copy (src/likelihood.c:7885-7889) */
     FlipSiteScalerSpace (m, chain);
-    sd->ev.site_scaler_dst = m->siteScalerIndex[chain];
-    sd->ev.site_scaler_src = (m->upDateAll == YES) ? MB200_NONE : m->siteScalerScratchIndex;
+    SeamSiteScalers (m, sd, chain);
 
     TreeTiProbs_Beagle (tree, d, chain);
     sd->guard = NO;
     /* (only inside chain-batched generations: their hooks are what can undo a retry's extra flips after a rejection) */
-    if (SeamDynamicRescaling () == YES && seamBatchQueue == YES && chain < sd->nSlots && m->numModelStates == 4 &&
-        (m->dataType == DNA || m->dataType == RNA) && sd->dynFreq[chain] > 1)
+    if (SeamDynamicRescaling () == YES && seamRun == SEAM_RUN_QUEUED && chain < sd->nSlots && m->numModelStates == 4 &&
+        (m->dataType == DNA || m->dataType == RNA) && sd->chains[chain].dynFreq > 1)
         {
-        /* 4-state divisions only (the kernels that carry the float-range guard, MB200_FLAG_RANGE_GUARD).
-           The chain's own rescale frequency steers the reference's bookkeeping fields (m->rescaleFreq is 1 in builds
-           without BEAGLE, src/mcmc.c:6157-6164) for the duration of the call */
-        const int savedFreq = m->rescaleFreq[chain];
-        m->rescaleFreq[chain] = sd->dynFreq[chain];
-        TreeCondLikes_Beagle_Always_Rescale (tree, d, chain);
-        m->rescaleFreq[chain] = savedFreq;
+        /* 4-state divisions only (the kernels that carry the float-range guard, MB200_FLAG_RANGE_GUARD): the built-in
+           path's policy at the chain's own rescale frequency */
+        SeamBuildOpsAtFrequency (tree, d, chain, SEAM_OPS_POLICY, sd->chains[chain].dynFreq);
         sd->guard = YES;
         }
     else
@@ -1352,7 +1405,7 @@ static int SeamDeviceEigenWanted (ModelInfo *m)
         const char *e = getenv ("MB200_EIGEN");
         mode = (e == NULL) ? 2 : (strcmp (e, "device") == 0) ? 1 : 0;
         }
-    if (mode == 0 || seamBackend.set_rate_matrices == NULL)
+    if (mode == 0 || seamBackend->set_rate_matrices == NULL)
         return NO;
     if (mode == 2 && m->numModelStates <= 32)
         return NO;
@@ -1443,12 +1496,12 @@ static int SeamDeviceEigen (ModelInfo *m, SeamDivision *sd, int d, int chain)
                 }
     FlipCijkSpace (m, chain);
     /* after the flip the scratch entry is the slot of the chain's pre-proposal state: a nearby eigensystem */
-    if (seamBackend.set_rate_matrices (sd->instance, m->cijkIndex[chain], m->cijkScratchIndex, seamQFlat[d], bs) != MB200_SUCCESS)
+    if (seamBackend->set_rate_matrices (sd->instance, m->cijkIndex[chain], m->cijkScratchIndex, seamQFlat[d], bs) != MB200_SUCCESS)
         {
         FlipCijkSpace (m, chain);       /* back; the host path flips again */
         return (NO);
         }
-    seamCijkSeen[d][m->cijkIndex[chain] >> 3] |= (unsigned char)(1 << (m->cijkIndex[chain] & 7));
+    SeamBitAssign (seamCijkSeen[d], m->cijkIndex[chain], YES);
     seamSecCijk += SeamNow () - t0;
     seamCijkUpdates++;
     seamDeviceEigens++;
@@ -1463,15 +1516,70 @@ static int SeamSyncCijk (ModelInfo *m, SeamDivision *sd, int d, int chain)
 
     if (idx < 0 || idx > 2 * MAX_CHAINS)
         return (ERROR);
-    if (m->upDateCijk == YES || (seamCijkSeen[d][idx >> 3] & (1 << (idx & 7))) == 0)
+    if (m->upDateCijk == YES || SeamBitGet (seamCijkSeen[d], idx) == 0)
         {
         double t0 = SeamNow ();
-        if (seamBackend.set_cijk (sd->instance, idx, m->cijks[idx]) != MB200_SUCCESS)
+        if (seamBackend->set_cijk (sd->instance, idx, m->cijks[idx]) != MB200_SUCCESS)
             return (ERROR);
         seamSecCijkUpload += SeamNow () - t0;
-        seamCijkSeen[d][idx >> 3] |= (unsigned char)(1 << (idx & 7));
+        SeamBitAssign (seamCijkSeen[d], idx, YES);
         }
     return (NO_ERROR);
+}
+
+/* The model-specific part of MB200LaunchLogLikeForDivision: puts the eigensystem the evaluation reads where the engine
+   looks for it (inline block, device slot, or none) and sets upDateAll like LaunchLogLikeForDivision
+   (src/likelihood.c:7864-7872).  READY: launch; FAILED: the move failed, lnL (and, where the reference does, abortMove)
+   are set; NOT_HANDLED: the division goes back to the reference's own path, nothing was flipped. */
+enum { SEAM_EIGEN_READY, SEAM_EIGEN_FAILED, SEAM_EIGEN_NOT_HANDLED };
+
+static int SeamPrepareEigen (ModelInfo *m, SeamDivision *sd, int d, int chain, MrBFlt *lnL)
+{
+    /* STANDARD data: the engine reads no eigensystem (equal-frequency Mk has none, cijkLength == 0; the others' matrices
+       come from TiProbs_Std), but the reference's driver still calls UpDateCijk when flagged (src/likelihood.c:7864) -- a
+       no-op for Mk -- and so does the seam; SeamDeviceEigenWanted is NO for these divisions */
+    const int hasEigen = (m->dataType != STANDARD) ? YES : NO;
+    int       deviceEigen = NO;
+
+    sd->inlineEigen = MB200SeamClosedFormModel (m);
+    if (sd->inlineEigen == YES)
+        {
+        /* no cijk bookkeeping in the reference for these models: derive the eigensystem of the
+           chain's current kappa / base frequencies and send it along with the evaluation */
+        if (m->upDateCijk == YES)
+            m->upDateAll = YES;
+        if (SeamClosedFormEigen (m, chain, sd->eigenBlock) == ERROR)
+            {
+            SeamFailMove (lnL);
+            return SEAM_EIGEN_FAILED;
+            }
+        return SEAM_EIGEN_READY;
+        }
+
+    /* every reason to hand the division back to the reference's own path comes BEFORE UpDateCijk:
+       that call flips the cijk space, and a second UpDateCijk by the fallback path would overwrite
+       the slot ResetFlips needs to restore a rejected move (src/mcmc.c:15695) */
+    if (hasEigen == YES && (m->cijkIndex[chain] < 0 || m->cijkIndex[chain] > 2 * MAX_CHAINS ||
+                            m->cijkScratchIndex < 0 || m->cijkScratchIndex > 2 * MAX_CHAINS))
+        return SEAM_EIGEN_NOT_HANDLED;
+
+    if (m->upDateCijk == YES)
+        {
+        if (SeamDeviceEigenWanted (m) == YES && SeamDeviceEigen (m, sd, d, chain) == YES)
+            deviceEigen = YES;
+        else if (SeamUpDateCijk (d, chain) == ERROR)
+            {
+            (*lnL) = MRBFLT_NEG_MAX;        /* abortMove stays as it is: what LaunchLogLikeForDivision does (src/likelihood.c:7864-7872) */
+            return SEAM_EIGEN_FAILED;
+            }
+        m->upDateAll = YES;
+        }
+    if (hasEigen == YES && deviceEigen == NO && SeamSyncCijk (m, sd, d, chain) == ERROR)
+        {
+        SeamFailMove (lnL);
+        return SEAM_EIGEN_FAILED;
+        }
+    return SEAM_EIGEN_READY;
 }
 
 /* ---- replacement for LaunchLogLikeForDivision (src/likelihood.c:7851) -------------- */
@@ -1479,114 +1587,42 @@ static int SeamSyncCijk (ModelInfo *m, SeamDivision *sd, int d, int chain)
    reference's own function-pointer path for it). */
 int MB200LaunchLogLikeForDivision (int chain, int d, MrBFlt *lnL)
 {
-    ModelInfo  *m;
-    Tree       *tree;
+    ModelInfo    *m;
     SeamDivision *sd;
-    int         deviceEigen;
+    int           eigen;
 
     SeamInit ();
     m = &modelSettings[d];
     if (MB200SeamDivisionSupported (m) == NO)
         return (NO);
     sd = &seamDiv[d];
-    if (sd->instance >= 0 &&
-        (sd->parsPtr != (const void *) m->parsSets || sd->weightPtr != (const void *) numSitesOfPat ||
-         sd->cfg.pattern_count != m->numChars || sd->cfg.category_count != SeamCategories (m) ||
-         sd->cfg.partials_count != m->numCondLikes + sd->extraCl || sd->cfg.matrix_count != m->numTiProbs + sd->extraTi ||
-         sd->cfg.scaler_count != m->numScalers + sd->extraNs || (m->dataType != STANDARD && sd->cfg.state_count != m->numModelStates) ||
-         sd->cfg.weight_rows != chainParams.numChains || sd->cfg.eigen_count != numLocalChains + 1 + sd->extraEig))
-        {
-        /* another mcmc run in the same session (new model, character set or chain count): the cached
-           instance is checked against the current model and rebuilt when it no longer matches */
-        if (InitBeagleInstance (m, d) == ERROR)
-            return (NO);
-        }
-    if (sd->instance < 0 && InitBeagleInstance (m, d) == ERROR)
+    if ((sd->instance < 0 || SeamInstanceStale (m, sd) == YES) && InitBeagleInstance (m, d) == ERROR)
         return (NO);
 
-    tree = GetTree (m->brlens, chain, state[chain]);
-
-    if (MB200SeamClosedFormModel (m) == YES)
-        {
-        /* no cijk bookkeeping in the reference for these models: derive the eigensystem of the
-           chain's current kappa / base frequencies and send it along with the evaluation */
-        sd->inlineEigen = YES;
-        if (m->upDateCijk == YES)
-            m->upDateAll = YES;                 /* what LaunchLogLikeForDivision does (src/likelihood.c:7864-7872) */
-        if (SeamClosedFormEigen (m, chain, sd->eigenBlock) == ERROR)
-            {
-            (*lnL) = MRBFLT_NEG_MAX;
-            abortMove = YES;
-            return (YES);
-            }
-        LaunchBEAGLELogLikeForDivision (chain, d, m, tree, lnL);
-        return (YES);
-        }
-    sd->inlineEigen = NO;
-
-    if (m->dataType == STANDARD)
-        {
-        /* equal-frequency Mk: no eigensystem (cijkLength == 0); the reference's driver would still call
-           UpDateCijk when flagged (src/likelihood.c:7864), which is a no-op for these models */
-        if (m->upDateCijk == YES)
-            {
-            if (SeamUpDateCijk (d, chain) == ERROR)
-                {
-                (*lnL) = MRBFLT_NEG_MAX;
-                return (YES);
-                }
-            m->upDateAll = YES;
-            }
-        LaunchBEAGLELogLikeForDivision (chain, d, m, tree, lnL);
-        return (YES);
-        }
-
-    /* every reason to hand the division back to the reference's own path comes BEFORE UpDateCijk:
-       that call flips the cijk space, and a second UpDateCijk by the fallback path would overwrite
-       the slot ResetFlips needs to restore a rejected move (src/mcmc.c:15695) */
-    if (m->cijkIndex[chain] < 0 || m->cijkIndex[chain] > 2 * MAX_CHAINS ||
-        m->cijkScratchIndex < 0 || m->cijkScratchIndex > 2 * MAX_CHAINS)
+    eigen = SeamPrepareEigen (m, sd, d, chain, lnL);
+    if (eigen == SEAM_EIGEN_NOT_HANDLED)
         return (NO);
-
-    deviceEigen = NO;
-    if (m->upDateCijk == YES)
-        {
-        if (SeamDeviceEigenWanted (m) == YES && SeamDeviceEigen (m, sd, d, chain) == YES)
-            deviceEigen = YES;
-        else if (SeamUpDateCijk (d, chain) == ERROR)
-            {
-            (*lnL) = MRBFLT_NEG_MAX;    /* effectively abort the move */
-            return (YES);
-            }
-        m->upDateAll = YES;
-        }
-    if (deviceEigen == NO && SeamSyncCijk (m, sd, d, chain) == ERROR)
-        {
-        (*lnL) = MRBFLT_NEG_MAX;
-        abortMove = YES;
-        return (YES);
-        }
-
-    LaunchBEAGLELogLikeForDivision (chain, d, m, tree, lnL);
+    if (eigen == SEAM_EIGEN_READY)
+        LaunchBEAGLELogLikeForDivision (chain, d, m, GetTree (m->brlens, chain, state[chain]), lnL);
     return (YES);
 }
 
-/* collect the result of a deferred evaluation of division d */
-static int SeamCollect (int d, int chain, MrBFlt *lnL)
+/* collect the results of the deferred evaluations of the listed divisions (divisions == NULL: divisions 0 .. n-1) */
+static void SeamCollect (const int *divisions, int n, int chain)
 {
-    SeamDivision *sd = &seamDiv[d];
-    double        value = 0.0;
-    int           status = MB200_EVAL_OK, rc = sd->syncRc;
+    int           i, d;
+    SeamDivision *sd;
 
-    sd->pending = NO;
-    if (seamBackend.evaluate_begin != NULL && seamBackend.evaluate_end != NULL)
+    for (i=0; i<n; i++)
         {
-        if (rc == MB200_SUCCESS)
-            rc = seamBackend.evaluate_end (sd->instance, &value, &status);
+        d = (divisions != NULL) ? divisions[i] : i;
+        if (d >= SEAM_MAX_DIVISIONS || seamDiv[d].pending == NO)
+            continue;
+        sd = &seamDiv[d];
+        sd->pending = NO;
+        SeamFinish (sd);
+        SeamApplyResult (d, chain, sd->qRc, sd->qLnL[0], sd->qStatus[0], &(modelSettings[d].lnLike[2*chain + state[chain]]));
         }
-    else
-        { value = sd->syncValue; status = sd->syncStatus; }
-    return SeamApplyResult (d, chain, rc, value, status, lnL);
 }
 
 /* ---- replacement for the division loop of LogLike (src/mcmc.c:7421-7441) ------------ */
@@ -1597,7 +1633,7 @@ MrBFlt MB200LogLike (int chain, void (*cpuPath) (int chain, int d, MrBFlt *lnL))
     MrBFlt      chainLnLike = 0.0;
 
     /* pass 1: launch every division that needs updating (engine) or compute it (reference path) */
-    seamDeferred = YES;
+    seamRun = SEAM_RUN_DEFERRED;
     for (d=0; d<numCurrentDivisions; d++)
         {
         m = &modelSettings[d];
@@ -1605,20 +1641,15 @@ MrBFlt MB200LogLike (int chain, void (*cpuPath) (int chain, int d, MrBFlt *lnL))
             continue;
         if (MB200LaunchLogLikeForDivision (chain, d, &(m->lnLike[2*chain + state[chain]])) == NO)
             {
-            seamDeferred = NO;
+            seamRun = SEAM_RUN_NOW;     /* the reference's path may reach the function-pointer forms */
             cpuPath (chain, d, &(m->lnLike[2*chain + state[chain]]));
-            seamDeferred = YES;
+            seamRun = SEAM_RUN_DEFERRED;
             }
         }
-    seamDeferred = NO;
+    seamRun = SEAM_RUN_NOW;
 
     /* pass 2: collect */
-    for (d=0; d<numCurrentDivisions; d++)
-        {
-        m = &modelSettings[d];
-        if (d < SEAM_MAX_DIVISIONS && seamDiv[d].pending == YES)
-            SeamCollect (d, chain, &(m->lnLike[2*chain + state[chain]]));
-        }
+    SeamCollect (NULL, numCurrentDivisions, chain);
     if (abortMove == YES)
         return MRBFLT_NEG_MAX;
     for (d=0; d<numCurrentDivisions; d++)
@@ -1693,9 +1724,9 @@ void MB200BatchEnterChain (int chain, int phase)
         if (phase == 1)
             {
             /* the division flags as this chain's move left them (ResetFlips reads them) */
-            m->upDateCl   = (seamFlagCl  [chain][d >> 3] >> (d & 7)) & 1 ? YES : NO;
-            m->upDateCijk = (seamFlagCijk[chain][d >> 3] >> (d & 7)) & 1 ? YES : NO;
-            m->upDateAll  = (seamFlagAll [chain][d >> 3] >> (d & 7)) & 1 ? YES : NO;
+            m->upDateCl   = SeamBitGet (seamFlagCl  [chain], d) ? YES : NO;
+            m->upDateCijk = SeamBitGet (seamFlagCijk[chain], d) ? YES : NO;
+            m->upDateAll  = SeamBitGet (seamFlagAll [chain], d) ? YES : NO;
             }
         }
 }
@@ -1709,25 +1740,25 @@ void MB200BatchLeaveChain (int chain, int phase)
         ModelInfo *m = &modelSettings[d];
         if (phase == 0)
             {
-            unsigned char bit = (unsigned char)(1 << (d & 7));
-            if (m->upDateCl   == YES) seamFlagCl  [chain][d >> 3] |= bit; else seamFlagCl  [chain][d >> 3] &= (unsigned char) ~bit;
-            if (m->upDateCijk == YES) seamFlagCijk[chain][d >> 3] |= bit; else seamFlagCijk[chain][d >> 3] &= (unsigned char) ~bit;
-            if (m->upDateAll  == YES) seamFlagAll [chain][d >> 3] |= bit; else seamFlagAll [chain][d >> 3] &= (unsigned char) ~bit;
+            SeamBitAssign (seamFlagCl  [chain], d, m->upDateCl   == YES);
+            SeamBitAssign (seamFlagCijk[chain], d, m->upDateCijk == YES);
+            SeamBitAssign (seamFlagAll [chain], d, m->upDateAll  == YES);
             }
-        if (phase == 1 && chain < seamDiv[d].nSlots && seamDiv[d].nExtraFlip != NULL && seamDiv[d].nExtraFlip[chain] > 0)
+        if (phase == 1 && chain < seamDiv[d].nSlots && seamDiv[d].chains[chain].nExtraFlip > 0)
             {
             /* a retry (dynamic rescaling) flipped nodes the move had not touched; ResetFlips knows nothing of them:
                the move was rejected (state[chain] is back at its pre-proposal value) -> flip them back here */
             SeamDivision *sd = &seamDiv[d];
+            SeamChain    *ch = &sd->chains[chain];
             int           i;
-            if (state[chain] != sd->queuedState[chain])
-                for (i=0; i<sd->nExtraFlip[chain]; i++)
+            if (state[chain] != ch->queuedState)
+                for (i=0; i<ch->nExtraFlip; i++)
                     {
                     const int node = sd->extraFlip[(size_t)chain * sd->capOps + i];
                     FlipCondLikeSpace (m, chain, node);
                     FlipNodeScalerSpace (m, chain, node);
                     }
-            sd->nExtraFlip[chain] = 0;
+            ch->nExtraFlip = 0;
             }
         SeamRestoreScratch (m, &seamDiv[d]);
         }
@@ -1739,21 +1770,18 @@ void MB200BatchQueueLogLike (int chain)
     int         d;
     ModelInfo  *m;
 
-    seamBatchQueue = YES;
+    seamRun = SEAM_RUN_QUEUED;
     for (d=0; d<numCurrentDivisions; d++)
         {
         m = &modelSettings[d];
         if (m->upDateCl != YES)
             continue;
         if (MB200LaunchLogLikeForDivision (chain, d, &(m->lnLike[2*chain + state[chain]])) == NO)
-            {
-            m->lnLike[2*chain + state[chain]] = MRBFLT_NEG_MAX;       /* cannot happen after MB200BatchBegin's check */
-            abortMove = YES;
-            }
+            SeamFailMove (&(m->lnLike[2*chain + state[chain]]));      /* cannot happen after MB200BatchBegin's check */
         if (abortMove == YES)
             break;
         }
-    seamBatchQueue = NO;
+    seamRun = SEAM_RUN_NOW;
 }
 
 /* one device call per division for the whole generation; the divisions overlap on the device */
@@ -1761,26 +1789,18 @@ void MB200BatchFlush (void)
 {
     int           d;
     SeamDivision *sd;
-    const int     split = (seamBackend.evaluate_begin != NULL && seamBackend.evaluate_end != NULL) ? YES : NO;
 
     for (d=0; d<numCurrentDivisions; d++)
         {
         sd = &seamDiv[d];
         if (sd->nQueued == 0)
             continue;
-        if (split == YES)
-            sd->qRc = seamBackend.evaluate_begin (sd->instance, sd->qEv, sd->nQueued);
-        else
-            sd->qRc = seamBackend.evaluate (sd->instance, sd->qEv, sd->nQueued, sd->qLnL, sd->qStatus);
+        SeamStart (sd, sd->qEv, sd->nQueued);
         sd->qLaunched = YES;
         }
-    if (split == YES)
-        for (d=0; d<numCurrentDivisions; d++)
-            {
-            sd = &seamDiv[d];
-            if (sd->nQueued > 0 && sd->qRc == MB200_SUCCESS)
-                sd->qRc = seamBackend.evaluate_end (sd->instance, sd->qLnL, sd->qStatus);
-            }
+    for (d=0; d<numCurrentDivisions; d++)
+        if (seamDiv[d].nQueued > 0)
+            SeamFinish (&seamDiv[d]);
 }
 
 /* phase B: the chain's log likelihood, with LogLike's conventions */
@@ -1816,7 +1836,7 @@ void LaunchBEAGLELogLikeMultiPartition (int *divisions, int divisionCount, int c
     ModelInfo  *m;
 
     (*lnL) = 0.0;
-    seamDeferred = YES;
+    seamRun = SEAM_RUN_DEFERRED;
     for (i=0; i<divisionCount; i++)
         {
         d = divisions[i];
@@ -1829,20 +1849,14 @@ void LaunchBEAGLELogLikeMultiPartition (int *divisions, int divisionCount, int c
         if (MB200LaunchLogLikeForDivision (chain, d, &(m->lnLike[2*chain + state[chain]])) == NO)
             {
             MrBayesPrint ("%s   H100 engine: division %d is outside the engine's coverage\n", spacer, d+1);
-            m->lnLike[2*chain + state[chain]] = MRBFLT_NEG_MAX;
-            abortMove = YES;
+            SeamFailMove (&(m->lnLike[2*chain + state[chain]]));
             }
         m->upDateCijk = hadCijk;
         }
-    seamDeferred = NO;
+    seamRun = SEAM_RUN_NOW;
+    SeamCollect (divisions, divisionCount, chain);
     for (i=0; i<divisionCount; i++)
-        {
-        d = divisions[i];
-        m = &modelSettings[d];
-        if (d < SEAM_MAX_DIVISIONS && seamDiv[d].pending == YES)
-            SeamCollect (d, chain, &(m->lnLike[2*chain + state[chain]]));
-        (*lnL) += m->lnLike[2*chain + state[chain]];
-        }
+        (*lnL) += modelSettings[divisions[i]].lnLike[2*chain + state[chain]];
     if (abortMove == YES)
         (*lnL) = MRBFLT_NEG_MAX;
 }
@@ -1882,27 +1896,14 @@ int TiProbs_B200 (TreeNode *p, int division, int chain)
 {
     ModelInfo           *m  = &modelSettings[division];
     SeamDivision        *sd = &seamDiv[division];
-    mb200_matrix_update *u;
 
     if (sd->instance < 0)
         return (ERROR);
     SeamOpenRecord (sd, m, chain);
-    if (sd->stdHostP == YES)
-        {
-        const int idx = m->tiProbsIndex[chain][p->index];
-        if (TiProbs_Std (p, division, chain) == ERROR ||
-            seamBackend.set_transition_matrix (sd->instance, idx, m->tiProbs[idx]) != MB200_SUCCESS)
-            return (ERROR);
-        return (NO_ERROR);
-        }
-    if (sd->ev.matrix_update_count >= sd->capMats)
+    if (sd->stdHostP == NO && sd->ev.matrix_update_count >= sd->capMats)
         return (ERROR);
     /* the caller has flipped the branch's slot already (src/likelihood.c:7899) */
-    u = &sd->mats[sd->ev.matrix_update_count++];
-    u->matrix = m->tiProbsIndex[chain][p->index];
-    u->eigen  = (sd->inlineEigen == YES) ? MB200_EIGEN_INLINE : (m->dataType == STANDARD) ? MB200_NONE : m->cijkIndex[chain];
-    u->length = SeamBranchLength (m, p, chain);
-    return (NO_ERROR);
+    return SeamMatrixRecord (m, sd, p, chain);
 }
 
 static int SeamRecordNode (TreeNode *p, int division, int chain, int isRoot)
@@ -1918,19 +1919,11 @@ static int SeamRecordNode (TreeNode *p, int division, int chain, int isRoot)
         return (ERROR);
     op = &sd->ops[sd->ev.operation_count++];
     FlipCondLikeSpace (m, chain, p->index);
-    op->dest    = m->condLikeIndex[chain][p->index];
-    op->child1  = m->condLikeIndex[chain][p->left->index];
-    op->matrix1 = m->tiProbsIndex [chain][p->left->index];
-    op->child2  = m->condLikeIndex[chain][p->right->index];
-    op->matrix2 = m->tiProbsIndex [chain][p->right->index];
-    op->child3  = (isRoot == YES) ? m->condLikeIndex[chain][p->anc->index] : MB200_NONE;
-    op->matrix3 = (isRoot == YES) ? m->tiProbsIndex [chain][p->index]      : MB200_NONE;
+    SeamOpRecord (m, sd, op, p, chain, isRoot);
     /* the caller removes the node's old scaler right after this call when this holds
        (src/likelihood.c:7938) and flips the node-scaler space after that (:7959) */
-    op->scale_remove = (m->unscaledNodes[chain][p->index] == 0 && m->upDateAll == NO)
-                     ? m->nodeScalerIndex[chain][p->index] : MB200_NONE;
+    op->scale_remove = SeamScaleRemove (m, p, chain);
     op->scale_write  = MB200_NONE;
-    sd->clUpdates += (long long) m->numChars * SeamCategories (m);
     return (NO_ERROR);
 }
 
@@ -1973,15 +1966,10 @@ int Likelihood_B200 (TreeNode *p, int division, int chain, MrBFlt *lnL, int whic
     SeamOpenRecord (sd, m, chain);          /* nothing dirty: root integration alone */
     sd->recording = NO;
     /* the caller has flipped the site-scaler space and reset or copied it (src/likelihood.c:7885-7889) */
-    sd->ev.site_scaler_dst = m->siteScalerIndex[chain];
-    sd->ev.site_scaler_src = (m->upDateAll == YES) ? MB200_NONE : m->siteScalerScratchIndex;
-    if (sd->inlineEigen == YES)
-        {
-        if (SeamClosedFormEigen (m, chain, sd->eigenBlock) == ERROR)
-            { (*lnL) = MRBFLT_NEG_MAX; abortMove = YES; return (ERROR); }
-        }
-    else if (m->dataType != STANDARD && SeamSyncCijk (m, sd, division, chain) == ERROR)
-        { (*lnL) = MRBFLT_NEG_MAX; abortMove = YES; return (ERROR); }
+    SeamSiteScalers (m, sd, chain);
+    if ((sd->inlineEigen == YES) ? SeamClosedFormEigen (m, chain, sd->eigenBlock) == ERROR
+                                 : (m->dataType != STANDARD && SeamSyncCijk (m, sd, division, chain) == ERROR))
+        return SeamFailMove (lnL);
     SeamCategoryRates (m, sd, division, chain);
     return SeamRootAndLaunch (division, chain, p->index, lnL, whichSitePats);
 }
@@ -2080,12 +2068,12 @@ static int SeamSyncHost (int division, int chain)
         {
         p = t->allDownPass[i];
         if (p->left != NULL && p->right != NULL)
-            rc = seamBackend.get_partials (sd->instance, m->condLikeIndex[chain][p->index], m->condLikes[m->condLikeIndex[chain][p->index]]);
+            rc = seamBackend->get_partials (sd->instance, m->condLikeIndex[chain][p->index], m->condLikes[m->condLikeIndex[chain][p->index]]);
         if (rc == MB200_SUCCESS && p->anc != NULL && m->tiProbsIndex[chain][p->index] >= 0)
-            rc = seamBackend.get_transition_matrix (sd->instance, m->tiProbsIndex[chain][p->index], m->tiProbs[m->tiProbsIndex[chain][p->index]]);
+            rc = seamBackend->get_transition_matrix (sd->instance, m->tiProbsIndex[chain][p->index], m->tiProbs[m->tiProbsIndex[chain][p->index]]);
         }
     if (rc == MB200_SUCCESS)
-        rc = seamBackend.get_scalers (sd->instance, m->siteScalerIndex[chain], m->scalers[m->siteScalerIndex[chain]]);
+        rc = seamBackend->get_scalers (sd->instance, m->siteScalerIndex[chain], m->scalers[m->siteScalerIndex[chain]]);
     if (rc != MB200_SUCCESS)
         {
         MrBayesPrint ("%s   H100 engine: cannot read the buffers of division %d back (%s)\n", spacer, division+1, mb200_error_string (rc));
@@ -2135,7 +2123,7 @@ static int SeamSyncRootPartials (TreeNode *p, int division, int chain)
     if (sd->instance < 0 || m->condLikes == NULL || SeamHostBuffersFor (m, sd) == ERROR)
         return (ERROR);
     idx = m->condLikeIndex[chain][p->index];
-    if (seamBackend.get_partials (sd->instance, idx, m->condLikes[idx]) != MB200_SUCCESS)
+    if (seamBackend->get_partials (sd->instance, idx, m->condLikes[idx]) != MB200_SUCCESS)
         return (ERROR);
     return (NO_ERROR);
 }
