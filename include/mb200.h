@@ -317,6 +317,8 @@ int mb200_replay_results   (int instance, int batch, double *lnL, int *status);
  * instance, mb200_synchronize, or about 100 us without a new mb200_replay_begin. */
 int mb200_replay_begin     (int instance, int batch);
 int mb200_replay_end       (int instance, double *lnL, int *status);
+/* A batch whose replay_begin has not been collected by replay_end yet cannot be freed: the call
+ * returns MB200_ERROR_OUT_OF_RANGE, the code replay_begin uses for one evaluation in flight. */
 int mb200_free_batch       (int instance, int batch);
 int mb200_synchronize      (int instance);
 /* the CUDA stream (cudaStream_t as void*) all work of the instance is issued on, so a

@@ -18,25 +18,92 @@
 #include <time.h>
 #include <stdlib.h>
 #include <string.h>
+#include <memory>
 #include <mutex>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 namespace {
 
+// ---- resource owners: each frees what it holds when it is destroyed or assigned over, and reads as the raw
+// pointer or handle it holds, which DevCtx, kernel arguments and runtime calls take as views
+
+// a runtime call's error as an MB200 code (allocation errors are not sticky: cleared here)
+int rcOf (cudaError_t e)
+{
+    if (e != cudaSuccess) cudaGetLastError ();
+    return (e == cudaSuccess) ? MB200_SUCCESS : (e == cudaErrorMemoryAllocation) ? MB200_ERROR_OUT_OF_MEMORY : MB200_ERROR_CUDA;
+}
+
+template <class T, bool HOST>      // HOST: pinned host memory, else device memory
+struct Array
+{
+    T *p = nullptr;
+    Array () = default;
+    Array (Array &&o) noexcept : p (std::exchange (o.p, nullptr)) {}
+    Array &operator= (Array &&o) noexcept { std::swap (p, o.p); return *this; }
+    ~Array () { if (p) { if (HOST) cudaFreeHost (p); else cudaFree (p); } }
+    operator T * () const { return p; }
+    int alloc (size_t n, unsigned hostFlags = cudaHostAllocDefault)    // n elements in place of the old ones, none on failure
+    {
+        *this = Array ();
+        const int rc = rcOf (HOST ? cudaHostAlloc ((void **)&p, n * sizeof(T), hostFlags) : cudaMalloc ((void **)&p, n * sizeof(T)));
+        if (rc != MB200_SUCCESS) p = nullptr;
+        return rc;
+    }
+};
+template <class T> using DevArray = Array<T, false>;
+template <class T> using PinnedArray = Array<T, true>;
+
+template <class T>
+struct MappedArray : PinnedArray<T>    // pinned host memory the device reaches through `dev`
+{
+    T *dev = nullptr;
+    int alloc (size_t n)
+    {
+        int rc = PinnedArray<T>::alloc (n, cudaHostAllocMapped);
+        if (rc == MB200_SUCCESS) rc = rcOf (cudaHostGetDevicePointer ((void **)&dev, this->p, 0));
+        if (rc != MB200_SUCCESS) *this = MappedArray ();
+        return rc;
+    }
+};
+
+template <class H, cudaError_t (*Destroy) (H)>
+struct Handle                      // a stream or an event
+{
+    H h = nullptr;
+    Handle () = default;
+    Handle (Handle &&o) noexcept : h (std::exchange (o.h, nullptr)) {}
+    ~Handle () { if (h) Destroy (h); }
+    operator H () const { return h; }
+};
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
+
+// n events in place of `out`'s, all created or `out` unchanged
+int makeEvents (std::vector<Event> &out, int n, unsigned flags)
+{
+    std::vector<Event> ev (n);
+    int rc = MB200_SUCCESS;
+    for (int i = 0; i < n && rc == MB200_SUCCESS; i++)
+        rc = rcOf (cudaEventCreateWithFlags (&ev[i].h, flags));
+    if (rc == MB200_SUCCESS) out = std::move (ev);
+    return rc;
+}
+
 struct Batch                       // packed evaluations (device job format)
 {
-    char   *hBlob  = nullptr;      // pinned host copy
-    char   *dBlob  = nullptr;      // device copy
+    PinnedArray<char> hBlob;       // pinned host copy
+    DevArray<char> dBlob;          // device copy
     size_t  cap    = 0;            // bytes allocated
     size_t  bytes  = 0;            // bytes used
     int     nEval = 0, nMat = 0, nOp = 0, nDbl = 0;
     size_t  offEval = 0, offDbl = 0, offUpd = 0, offChunk = 0, offCmat = 0, offOp = 0, offOrd = 0;
     int     maxOps = 0;            // most operations of any evaluation (tensor-core path: work-queue geometry)
-    DevResult *dRes = nullptr;     // [capEval] results in HBM (device-resident replay)
-    DevResult *hRes = nullptr;     // [capEval] pinned + mapped: kernels of the host-call path write
+    DevArray<DevResult> dRes;      // [capEval] results in HBM (device-resident replay)
+    MappedArray<DevResult> hRes;   // [capEval] pinned + mapped: kernels of the host-call path write
                                    // results straight into host memory, the caller polls `seq`
-    DevResult *hResDev = nullptr;  // device alias of hRes
     int     capEval = 0;
     int     nDirty = 0;            // P(t) rebuilds in the batch
     bool    fused = false;         // 4-state latency path: P(t) rebuilt inside the pruning kernel
@@ -58,42 +125,58 @@ struct Pending                     // the evaluation begin() started and end() h
     int     tiles = 1;             // tiles per evaluation (host sum only)
 };
 
+struct EigenSolver                     // device eigensolver staging (mb200_set_rate_matrices), built on first use
+{
+    size_t        inStride = 0;        // doubles per slot: [parts x S x S rate matrices | S frequencies]
+    DevArray<double> dIn; PinnedArray<double> hIn;     // the staging area on the device and its pinned host copy
+    MappedArray<int> status;           // non-zero = the Jacobi iteration did not converge
+    DevArray<double> vec;              // [slot][part][V | V^-1], unless dFactor (which the P(t) kernel wants anyway) holds them
+    DevArray<double> U;                // [slot][part][N x N] orthogonal eigenvectors of the symmetrised matrix (warm starts)
+    DevArray<double2> log; DevArray<int> rounds;       // [part] rotation log and rounds of the solve in flight (stream-ordered reuse)
+    std::vector<int> warmChain;        // per slot: -1 = no device eigenvectors, else warm starts since the last cold one
+    std::vector<Event> evIn;           // per slot: the staging area has been read
+};
+
+struct MatRing                         // pinned ring for caller-supplied transition matrices (copied without a host wait)
+{
+    PinnedArray<float> buf;            // MAT_RING slots of `stride` floats
+    std::vector<Event> ev;             // per slot: its copy has left the ring
+    size_t        stride = 0;
+    int           next = 0;            // the slot of the next call, modulo MAT_RING
+};
+
+struct Mailbox                         // resident generation kernel (mb200_replay_begin / _end, eval_nuc4_resident_kernel)
+{
+    MappedArray<int4> mail;            // host -> device mailbox: MB200_RES_PIECES pieces
+    DevArray<ResidentJob> job;         // the leader CTA's copy of the current job
+};
+
 struct Instance
 {
+    Stream        stream;              // first: outlives every buffer its work may use
     mb200_instance_config cfg;
     DevCtx        ctx;
-    cudaStream_t  stream = nullptr;
-    uint8_t      *dTip8 = nullptr;
-    uint64_t     *dTip64 = nullptr;
-    int          *dTipPartAmbig = nullptr;
+    DevArray<uint8_t> dTip8;
+    DevArray<uint64_t> dTip64;
+    DevArray<int> dTipPartAmbig;
     int           seq = 0;               // launch sequence number stamped into results
-    float        *dSplit = nullptr;      // tensor-core path: pre-split (hi, lo) canonical images of every P(t)
+    DevArray<float> dSplit;              // tensor-core path: pre-split (hi, lo) canonical images of every P(t)
     int           tcS = 0;               // 20 or 61 when the wgmma kernel serves this instance, else 0
-    size_t        smemTc = 0;
-    float        *dPartials = nullptr, *dMatrices = nullptr, *dScalers = nullptr, *dWeights = nullptr;
-    double       *dEigen = nullptr;
-    unsigned int *dTcCounter = nullptr;  // tensor-core path: ticket counter of the node-parallel work queue (monotone)
+    DevArray<float> dPartials, dMatrices, dScalers, dWeights;
+    DevArray<double> dEigen;
+    DevArray<unsigned int> dTcCounter;   // tensor-core path: ticket counter of the node-parallel work queue (monotone)
     unsigned int  tcBase = 0;            // its value before the next launch's first ticket
-    int          *dTcFlags = nullptr;    // [maxEval][maxTiles][tcFlagStride] node-done flags (== launch sequence number)
-    int          *dTcError = nullptr;
-    int           tcFlagStride = 0, tcGrid = 0;
+    DevArray<int> dTcFlags;              // [maxEval][maxTiles][tcFlagStride] node-done flags (== launch sequence number)
+    DevArray<int> dTcError;
+    int           tcFlagStride = 0;
     int           tcpStages = 0;         // pipelined tensor-core kernel: operand-ring stages that fit (0: kernel not usable)
     size_t        tcpSmem = 0;
-    double       *dFactor = nullptr;    // large state counts: rank-one factors (U, W) of every eigensystem's c_ijk slices
-    // device eigensolver (mb200_set_rate_matrices): per slot [parts x S x S rate matrices | S frequencies]
-    double       *dEigIn = nullptr, *hEigIn = nullptr;     // device copy and its pinned staging
-    double       *dEigVec = nullptr;     // [slot][part][V | V^-1]; == dFactor where the P(t) kernel wants the factors anyway
-    double       *dEigU = nullptr;       // [slot][part][N x N] orthogonal eigenvectors of the symmetrised matrix (warm starts)
-    double2      *dEigLog = nullptr;     // [part] rotation log of the solve in flight (stream-ordered reuse)
-    int          *dEigRounds = nullptr;  // [part]
-    std::vector<int> eigWarmChain;       // per slot: -1 = no device eigenvectors, else warm starts since the last cold one
-    int          *hEigStatus = nullptr;  // mapped: non-zero = the Jacobi iteration did not converge
-    size_t        eigInStride = 0;
-    std::vector<cudaEvent_t> evEigIn;    // per slot: the staging area has been read
-    uint64_t     *dInvMask = nullptr;
-    double2      *dTilePartial = nullptr;
-    int          *dTileAbort = nullptr;
-    unsigned int *dTicket = nullptr;
+    DevArray<double> dFactor;            // large state counts: rank-one factors (U, W) of every eigensystem's c_ijk slices
+    EigenSolver   eig;
+    DevArray<uint64_t> dInvMask;
+    DevArray<double2> dTilePartial;
+    DevArray<int> dTileAbort;
+    DevArray<unsigned int> dTicket;
     bool          invMaskValid = false;
     int           maxEval = 1, maxTiles = 1, numSMs = 132;
     size_t        eigenStride = 0;     // doubles per eigen slot (all parts)
@@ -105,13 +188,8 @@ struct Instance
     int           writtenStamp = 0;
     Pending       pending;
     Batch         scratch;             // used by the synchronous entry points
-    std::vector<Batch *> batches;      // resident batches (mb200_pack_evaluations)
-    void         *hostStage = nullptr; // pinned staging for set/get calls
-    size_t        hostStageBytes = 0;
-    float        *hMatRing = nullptr;  // pinned ring for caller-supplied transition matrices (mb200_set_transition_matrix without a sync)
-    size_t        matRingStride = 0;
-    int           matRingNext = 0;
-    std::vector<cudaEvent_t> evMatRing;
+    std::vector<std::unique_ptr<Batch>> batches;   // resident batches (mb200_pack_evaluations)
+    MatRing       ring;
     std::vector<int> slotOf;           // scratch: matrix index -> shared-memory slot in the current evaluation
     std::vector<int> touched;          // scratch: matrices whose slotOf entry is set
     std::vector<int> dirtyOf;          // scratch: matrix index -> index in the evaluation's update list
@@ -121,17 +199,14 @@ struct Instance
     bool          stdReady = false;    // mb200_set_pattern_states done
     bool          stdUniformMk = true; // every matrix the engine builds is an equal-frequency Mk matrix
     StdCtx        sx;
-    int          *dStdTab = nullptr;   // nStates | tiIndex | bsIndex, [3][C]
-    int2         *dStdClasses = nullptr;
+    DevArray<int> dStdTab;             // nStates | tiIndex | bsIndex, [3][C]
+    DevArray<int2> dStdClasses;
     std::vector<int> hNStates, hTiIndex, hBsIndex;
     std::vector<size_t> hClOff;        // ragged host layout: offset of pattern c inside a category's block
     bool          timing = false;      // bracket the fused kernel with events
-    std::vector<cudaEvent_t> evA, evB; // ring of event pairs
+    std::vector<Event> evA, evB;       // ring of event pairs
     long long     evCount = 0;         // pairs recorded since the last read
-    // resident generation kernel (mb200_replay_begin / _end, eval_nuc4_resident_kernel)
-    int4         *hMail = nullptr;     // host -> device mailbox: pinned, mapped, MB200_RES_PIECES pieces
-    int4         *hMailDev = nullptr;  // its device alias
-    ResidentJob  *dJob = nullptr;      // the leader CTA's copy of the current job
+    Mailbox       res;
     bool          resOk = false;       // the resident kernel may serve this instance: 4-state, its grid fits the
                                        // device at once, and (once tried) its mailbox could be allocated
     bool          resident = false;    // a resident kernel may still run on the stream
@@ -193,47 +268,22 @@ int use (Instance *I)
     return retire (I);
 }
 
-int ensureStage (Instance *I, size_t bytes)
-{
-    if (bytes <= I->hostStageBytes)
-        return MB200_SUCCESS;
-    if (I->hostStage) cudaFreeHost (I->hostStage);
-    I->hostStage = nullptr; I->hostStageBytes = 0;
-    CK (cudaMallocHost (&I->hostStage, bytes));
-    I->hostStageBytes = bytes;
-    return MB200_SUCCESS;
-}
-
-void freeBatch (Batch &b)
-{
-    if (b.hBlob)   cudaFreeHost (b.hBlob);
-    if (b.dBlob)   cudaFree (b.dBlob);
-    if (b.dRes)    cudaFree (b.dRes);
-    if (b.hRes)    cudaFreeHost (b.hRes);
-    b = Batch ();
-}
-
 int reserveBatch (Batch &b, size_t bytes, int nEval)
 {
     if (bytes > b.cap)
         {
-        size_t cap = bytes + bytes / 2 + 32768;      // never smaller than the largest parameter blob
-        if (b.hBlob) cudaFreeHost (b.hBlob);
-        if (b.dBlob) cudaFree (b.dBlob);
-        b.hBlob = nullptr; b.dBlob = nullptr; b.cap = 0;
-        CK (cudaMallocHost ((void **)&b.hBlob, cap));
-        CK (cudaMalloc ((void **)&b.dBlob, cap));
+        const size_t cap = bytes + bytes / 2 + 32768;      // never smaller than the largest parameter blob
+        b.cap = 0;
+        int rc = b.hBlob.alloc (cap);
+        if (rc || (rc = b.dBlob.alloc (cap))) return rc;
         b.cap = cap;
         }
     if (nEval > b.capEval)
         {
-        int cap = nEval + 8;
-        if (b.dRes) cudaFree (b.dRes);
-        if (b.hRes) cudaFreeHost (b.hRes);
+        const int cap = nEval + 8;
         b.capEval = 0;
-        CK (cudaMalloc ((void **)&b.dRes, sizeof(DevResult) * cap));
-        CK (cudaHostAlloc ((void **)&b.hRes, sizeof(DevResult) * cap * HOSTSUM_MAX_TILES, cudaHostAllocMapped));
-        CK (cudaHostGetDevicePointer ((void **)&b.hResDev, b.hRes, 0));
+        int rc = b.dRes.alloc (cap);
+        if (rc || (rc = b.hRes.alloc ((size_t) cap * HOSTSUM_MAX_TILES))) return rc;
         memset (b.hRes, 0, sizeof(DevResult) * cap * HOSTSUM_MAX_TILES);
         b.capEval = cap;
         }
@@ -520,7 +570,7 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
     rc = reserveBatch (b, bytes, count);
     if (rc != MB200_SUCCESS)
         return rc;
-    DevBatchHeader *h = (DevBatchHeader *) b.hBlob;
+    DevBatchHeader *h = (DevBatchHeader *) b.hBlob.p;
     h->nEval = count; h->nMat = nUpd; h->nOp = nOp; h->nDbl = nDbl;
     DevEval  *de = (DevEval  *)(b.hBlob + offEval);
     double   *dd = (double   *)(b.hBlob + offDbl);
@@ -707,7 +757,7 @@ int launch (Instance *I, Batch &b, bool viaParams, bool toHost)
     const DevChunk *dc = (const DevChunk *)(b.dBlob + b.offChunk);
     const DevMat   *dm = (const DevMat   *)(b.dBlob + b.offCmat);
     const DevOp    *dops = (const DevOp  *)(b.dBlob + b.offOp);
-    DevResult *res = toHost ? b.hResDev : b.dRes;
+    DevResult *res = toHost ? b.hRes.dev : b.dRes;
     DevCtx ctx = I->ctx;
     const int seq = ++I->seq;
 
@@ -729,7 +779,7 @@ int launch (Instance *I, Batch &b, bool viaParams, bool toHost)
             dim3 grid (b.nMat, ctx.K);
             const int LD = (ctx.S + 3) & ~3;
             tiprobs_mm_kernel<<<grid, 256, (size_t)2 * ctx.S * LD * sizeof(double), I->stream>>> (ctx, de, b.nEval, dd, du, I->dFactor,
-                                                                                                   (I->tcS == 61) ? I->dSplit : nullptr);
+                                                                                                   (I->tcS == 61) ? I->dSplit.p : nullptr);
             }
         else
             {
@@ -777,7 +827,7 @@ int launch (Instance *I, Batch &b, bool viaParams, bool toHost)
                 {
                 constexpr int CAP = decltype (cap)::value;
                 eval_nuc4_pkernel<KK, NT_NUC4, CAP><<<grid, NT_NUC4, nuc4Smem<KK, true>, I->stream>>> (
-                    ctx, off, res, seq, b.jx, *reinterpret_cast<const ParamBlob<CAP> *>(b.hBlob));
+                    ctx, off, res, seq, b.jx, *reinterpret_cast<const ParamBlob<CAP> *>(b.hBlob.p));
                 };
             if (!viaParams && b.fused)
                 eval_nuc4_kernel<KK, NT_NUC4, true><<<grid, NT_NUC4, nuc4Smem<KK, true>, I->stream>>> (ctx, de, dd, dc, dm, dops, res, seq, b.jx);
@@ -859,7 +909,7 @@ void post (Instance *I, int seq, int count, const Batch *b)
     p[0].x = count;
     if (b)
         {
-        const unsigned long long blob = (unsigned long long) b->dBlob, res = (unsigned long long) b->hResDev;
+        const unsigned long long blob = (unsigned long long) b->dBlob.p, res = (unsigned long long) b->hRes.dev;
         p[0].y = (int)(unsigned) blob; p[0].z = (int)(unsigned)(blob >> 32);
         p[1].x = (int)(unsigned) res;  p[1].y = (int)(unsigned)(res >> 32); p[1].z = (int) b->offEval;
         p[2].x = (int) b->offDbl; p[2].y = (int) b->offChunk; p[2].z = (int) b->offCmat;
@@ -874,7 +924,7 @@ void post (Instance *I, int seq, int count, const Batch *b)
     for (int i = 0; i < nP; i++)
         {
         p[i].w = seq;
-        _mm_store_si128 (reinterpret_cast<__m128i *>(I->hMail + i), _mm_load_si128 (reinterpret_cast<const __m128i *>(p + i)));
+        _mm_store_si128 (reinterpret_cast<__m128i *>(I->res.mail.p + i), _mm_load_si128 (reinterpret_cast<const __m128i *>(p + i)));
         }
     __atomic_signal_fence (__ATOMIC_SEQ_CST);
 }
@@ -910,19 +960,14 @@ bool residentEligible (Instance *I, const Batch &b)
     if (live != 1)
         return false;
     }
-    if (!I->dJob)
+    if (!I->res.job)
         {
         // mailbox and job copy on first use; without them the instance keeps its launches
-        if (cudaHostAlloc ((void **)&I->hMail, sizeof(int4) * MB200_RES_PIECES, cudaHostAllocMapped) != cudaSuccess ||
-            cudaHostGetDevicePointer ((void **)&I->hMailDev, I->hMail, 0) != cudaSuccess ||
-            cudaMalloc ((void **)&I->dJob, sizeof(ResidentJob)) != cudaSuccess ||
-            cudaMemset (I->dJob, 0, sizeof(ResidentJob)) != cudaSuccess)
-            {
-            cudaGetLastError ();
-            I->resOk = false;
-            return false;
-            }
-        memset (I->hMail, 0, sizeof(int4) * MB200_RES_PIECES);
+        Mailbox m;
+        if (m.mail.alloc (MB200_RES_PIECES) || m.job.alloc (1) || rcOf (cudaMemset (m.job, 0, sizeof(ResidentJob))))
+            { I->resOk = false; return false; }
+        memset (m.mail, 0, sizeof(int4) * MB200_RES_PIECES);
+        I->res = std::move (m);
         }
     return true;
 }
@@ -951,7 +996,7 @@ int residentStart (Instance *I, Batch &b)
         int rc = withNuc4K (ctx.K, [&] (auto k)
             {
             constexpr int KK = decltype (k)::value;
-            eval_nuc4_resident_kernel<KK, NT_NUC4><<<grid, NT_NUC4, nuc4Smem<KK, true>, I->stream>>> (ctx, I->hMailDev, I->dJob, seq0, RES_IDLE_NS);
+            eval_nuc4_resident_kernel<KK, NT_NUC4><<<grid, NT_NUC4, nuc4Smem<KK, true>, I->stream>>> (ctx, I->res.mail.dev, I->res.job, seq0, RES_IDLE_NS);
             CK (cudaGetLastError ());
             return MB200_SUCCESS;
             });
@@ -1095,10 +1140,10 @@ int runEnd (Instance *I, double *lnL, int *status)
             if (status) status[e] = MB200_EVAL_OK;
             }
         }
-    if (I->hEigStatus && *(volatile int *) I->hEigStatus != 0)
+    if (I->eig.status && *(volatile int *) I->eig.status.p != 0)
         {
         // an eigensystem this launch (or an earlier one) read did not converge: nothing computed from it can be used
-        *(volatile int *) I->hEigStatus = 0;
+        *(volatile int *) I->eig.status.p = 0;
         fprintf (stderr, "mb200: device eigensolver did not converge\n");
         return MB200_ERROR_GENERAL;
         }
@@ -1112,32 +1157,34 @@ int runSync (Instance *I, const mb200_evaluation *evs, int count, double *lnL, i
     return runEnd (I, lnL, status);
 }
 
+// the eigensolver's staging into `out`, complete, or an error and `out` unchanged
+int makeEigenSolver (const Instance *I, EigenSolver &out)
+{
+    EigenSolver g;
+    const int S = I->cfg.state_count, parts = I->cijkParts, slots = I->cfg.eigen_count;
+    const size_t n2 = (size_t)S * S, N = (S + 1) & ~1;
+    g.inStride = (size_t)parts * n2 + S;
+    int rc = g.dIn.alloc (slots * g.inStride);
+    if (!rc) rc = g.hIn.alloc (slots * g.inStride);
+    if (!rc) rc = g.status.alloc (1);
+    if (!rc && !I->dFactor) rc = g.vec.alloc ((size_t)slots * parts * 2 * n2);
+    if (!rc) rc = g.U.alloc ((size_t)slots * parts * N * N);
+    if (!rc) rc = g.log.alloc ((size_t)parts * MB200_EIG_LOG_DOUBLES / 2);
+    if (!rc) rc = g.rounds.alloc (parts);
+    if (!rc) rc = makeEvents (g.evIn, slots, cudaEventDisableTiming);
+    if (!rc) rc = rcOf (cudaFuncSetAttribute (eigen_rotations_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) eigen_smem_bytes ()));
+    if (rc != MB200_SUCCESS) return rc;
+    *g.status.p = 0;
+    g.warmChain.assign (slots, -1);
+    out = std::move (g);
+    return MB200_SUCCESS;
+}
+
 void destroy (Instance *I)
 {
-    if (!I) return;
     cudaSetDevice (I->cfg.device);
     retire (I);
     if (I->stream) cudaStreamSynchronize (I->stream);
-    freeBatch (I->scratch);
-    for (Batch *b : I->batches) if (b) { freeBatch (*b); delete b; }
-    cudaFree (I->dTip8); cudaFree (I->dTip64); cudaFree (I->dTipPartAmbig); cudaFree (I->dSplit); cudaFree (I->dPartials); cudaFree (I->dMatrices);
-    cudaFree (I->dScalers); cudaFree (I->dWeights); cudaFree (I->dEigen); cudaFree (I->dFactor); cudaFree (I->dInvMask);
-    cudaFree (I->dTilePartial); cudaFree (I->dTileAbort); cudaFree (I->dTicket);
-    cudaFree (I->dStdTab); cudaFree (I->dStdClasses);
-    cudaFree (I->dTcCounter); cudaFree (I->dTcFlags); cudaFree (I->dTcError);
-    cudaFree (I->dEigIn); if (I->dEigVec != I->dFactor) cudaFree (I->dEigVec);
-    cudaFree (I->dEigU); cudaFree (I->dEigLog); cudaFree (I->dEigRounds);
-    if (I->hEigIn) cudaFreeHost (I->hEigIn);
-    if (I->hEigStatus) cudaFreeHost (I->hEigStatus);
-    for (cudaEvent_t e : I->evEigIn) cudaEventDestroy (e);
-    if (I->hostStage) cudaFreeHost (I->hostStage);
-    if (I->hMatRing) cudaFreeHost (I->hMatRing);
-    if (I->hMail) cudaFreeHost (I->hMail);
-    cudaFree (I->dJob);
-    for (cudaEvent_t e : I->evMatRing) cudaEventDestroy (e);
-    for (cudaEvent_t e : I->evA) cudaEventDestroy (e);
-    for (cudaEvent_t e : I->evB) cudaEventDestroy (e);
-    if (I->stream) cudaStreamDestroy (I->stream);
     delete I;
 }
 
@@ -1239,71 +1286,49 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
     else
     I->maxTiles = I->tcS ? (C + TC_MIN_ROWS - 1) / TC_MIN_ROWS + 1 : nuc4 ? (C + nuc4PatternsPerBlock (K) - 1) / nuc4PatternsPerBlock (K) : (C + TP - 1) / TP;
 
-#define ALLOC(ptr, bytes) do { cudaError_t e_ = cudaMalloc ((void **)&(ptr), (bytes)); if (e_ != cudaSuccess) { \
-        cudaGetLastError (); destroy (I); return (e_ == cudaErrorMemoryAllocation) ? MB200_ERROR_OUT_OF_MEMORY : MB200_ERROR_CUDA; } } while (0)
-    if (cudaStreamCreateWithFlags (&I->stream, cudaStreamNonBlocking) != cudaSuccess) { destroy (I); return MB200_ERROR_CUDA; }
-    ALLOC (I->dTip8,     (size_t)cfg->tip_count * C);
-    ALLOC (I->dTip64,    (size_t)cfg->tip_count * C * sizeof(uint64_t));
-    ALLOC (I->dTipPartAmbig, (size_t)cfg->tip_count * sizeof(int));
-    ALLOC (I->dPartials, nInt * K * C * Sp * sizeof(float));
-    ALLOC (I->dMatrices, (size_t)cfg->matrix_count * K * S * S * sizeof(float));
-    ALLOC (I->dScalers,  (size_t)cfg->scaler_count * C * sizeof(float));
-    ALLOC (I->dWeights,  (size_t)cfg->weight_rows * C * sizeof(float));
-    ALLOC (I->dEigen,    (size_t)cfg->eigen_count * I->eigenStride * sizeof(double));
-    if (S > 32)
+    // n elements of a, zeroed on the stream
+    auto make = [&] (auto &a, size_t n) { int r = a.alloc (n); return r ? r : rcOf (cudaMemsetAsync (a, 0, n * sizeof(*a.p), I->stream)); };
+    int rc = rcOf (cudaStreamCreateWithFlags (&I->stream.h, cudaStreamNonBlocking));
+    if (!rc) rc = make (I->dTip8,     (size_t)cfg->tip_count * C);
+    if (!rc) rc = make (I->dTip64,    (size_t)cfg->tip_count * C);
+    if (!rc) rc = make (I->dTipPartAmbig, (size_t)cfg->tip_count);
+    if (!rc) rc = make (I->dPartials, nInt * K * C * Sp);
+    if (!rc) rc = make (I->dMatrices, (size_t)cfg->matrix_count * K * S * S);
+    if (!rc) rc = make (I->dScalers,  (size_t)cfg->scaler_count * C);
+    if (!rc) rc = make (I->dWeights,  (size_t)cfg->weight_rows * C);
+    if (!rc) rc = make (I->dEigen,    (size_t)cfg->eigen_count * I->eigenStride);
+    if (!rc && S > 32)
         {
-        ALLOC (I->dFactor, (size_t)cfg->eigen_count * I->cijkParts * 2 * S * S * sizeof(double));
+        rc = make (I->dFactor, (size_t)cfg->eigen_count * I->cijkParts * 2 * S * S);
         const int LD = (S + 3) & ~3;
-        if (cudaFuncSetAttribute (tiprobs_mm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)2 * S * LD * sizeof(double))) != cudaSuccess)
-            { destroy (I); return MB200_ERROR_CUDA; }
+        if (!rc) rc = rcOf (cudaFuncSetAttribute (tiprobs_mm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)2 * S * LD * sizeof(double))));
         }
-    if (I->tcS)
+    if (!rc && I->tcS)
         {
         // warp-specialised pipelined kernel: one CTA per SM, as many operand-ring stages as fit
         const size_t fl = withTcS (I->tcS, [&] (auto s) { return tcSetup<decltype (s)::value> (I); });
-        if (I->tcpStages == 0)
-            { destroy (I); return MB200_ERROR_UNSUPPORTED; }     // cannot happen for K <= 4 on a 227 KB part
-        ALLOC (I->dSplit, (size_t)cfg->matrix_count * K * fl * sizeof(float));
-        cudaMemsetAsync (I->dSplit, 0, (size_t)cfg->matrix_count * K * fl * sizeof(float), I->stream);
         I->tcFlagStride = (int) nInt + 1;
         const size_t nFlags = (size_t) I->maxEval * ((size_t)(C + TC_MIN_ROWS - 1) / TC_MIN_ROWS + 1) * I->tcFlagStride;
-        ALLOC (I->dTcCounter, sizeof(unsigned int));
-        ALLOC (I->dTcError, sizeof(int));
-        ALLOC (I->dTcFlags, nFlags * sizeof(int));
-        cudaMemsetAsync (I->dTcCounter, 0, sizeof(unsigned int), I->stream);
-        cudaMemsetAsync (I->dTcError, 0, sizeof(int), I->stream);
-        cudaMemsetAsync (I->dTcFlags, 0, nFlags * sizeof(int), I->stream);
+        rc = I->tcpStages ? make (I->dSplit, (size_t)cfg->matrix_count * K * fl) : MB200_ERROR_UNSUPPORTED;  // 0 stages: not for K <= 4 on a 227 KB part
+        if (!rc) rc = make (I->dTcCounter, 1);
+        if (!rc) rc = make (I->dTcError, 1);
+        if (!rc) rc = make (I->dTcFlags, nFlags);
         }
-    ALLOC (I->dInvMask,  (size_t)C * sizeof(uint64_t));
-    ALLOC (I->dTilePartial, (size_t)I->maxEval * I->maxTiles * sizeof(double2));
-    ALLOC (I->dTileAbort,   (size_t)I->maxEval * I->maxTiles * sizeof(int));
-    ALLOC (I->dTicket,      (size_t)I->maxEval * sizeof(unsigned int));
+    if (!rc) rc = make (I->dInvMask,  (size_t)C);
+    if (!rc) rc = make (I->dTilePartial, (size_t)I->maxEval * I->maxTiles);
+    if (!rc) rc = make (I->dTileAbort,   (size_t)I->maxEval * I->maxTiles);
+    if (!rc) rc = make (I->dTicket,      (size_t)I->maxEval);
+    if (!rc && I->smemGen > 48*1024) rc = rcOf (cudaFuncSetAttribute (eval_gen_kernel<NT_GEN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) I->smemGen));
+    if (!rc && nuc4 && nuc4Setup (I)) rc = MB200_ERROR_CUDA;
+    if (!rc) rc = rcOf (cudaStreamSynchronize (I->stream));
+    if (rc != MB200_SUCCESS)
+        { destroy (I); return rc; }           // the half-built instance frees what it holds
     if (I->std)
         {
-        ALLOC (I->dStdTab,       (size_t)3 * C * sizeof(int));
-        ALLOC (I->dStdClasses,   (size_t)MB200_STD_MAX_STATES * sizeof(int2));
         memset (&I->sx, 0, sizeof(I->sx));
         I->sx.lanes = stdLanes;
         }
-#undef ALLOC
-    cudaMemsetAsync (I->dTip8, 0, (size_t)cfg->tip_count * C, I->stream);
-    cudaMemsetAsync (I->dTip64, 0, (size_t)cfg->tip_count * C * sizeof(uint64_t), I->stream);
-    cudaMemsetAsync (I->dTipPartAmbig, 0, (size_t)cfg->tip_count * sizeof(int), I->stream);
     I->tipPartAmbig.assign (cfg->tip_count, 0);
-    cudaMemsetAsync (I->dPartials, 0, nInt * K * C * Sp * sizeof(float), I->stream);
-    cudaMemsetAsync (I->dMatrices, 0, (size_t)cfg->matrix_count * K * S * S * sizeof(float), I->stream);
-    cudaMemsetAsync (I->dScalers, 0, (size_t)cfg->scaler_count * C * sizeof(float), I->stream);
-    cudaMemsetAsync (I->dWeights, 0, (size_t)cfg->weight_rows * C * sizeof(float), I->stream);
-    cudaMemsetAsync (I->dEigen, 0, (size_t)cfg->eigen_count * I->eigenStride * sizeof(double), I->stream);
-    cudaMemsetAsync (I->dTicket, 0, (size_t)I->maxEval * sizeof(unsigned int), I->stream);
-
-    if (I->smemGen > 48*1024)
-        {
-        if (cudaFuncSetAttribute (eval_gen_kernel<NT_GEN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) I->smemGen) != cudaSuccess)
-            { destroy (I); return MB200_ERROR_CUDA; }
-        }
-    if (nuc4 && nuc4Setup (I) != MB200_SUCCESS)
-        { destroy (I); return MB200_ERROR_CUDA; }
 
     DevCtx &x = I->ctx;
     memset (&x, 0, sizeof(x));
@@ -1317,8 +1342,6 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
     x.scalers = I->dScalers; x.eigen = I->dEigen; x.weights = I->dWeights; x.invMask = I->dInvMask;
     x.cijkParts = I->cijkParts; x.patternTiles = 0;
     x.tilePartial = I->dTilePartial; x.tileAbort = I->dTileAbort; x.ticket = I->dTicket;
-
-    if (cudaStreamSynchronize (I->stream) != cudaSuccess) { destroy (I); return MB200_ERROR_CUDA; }
 
     std::lock_guard<std::mutex> g (gLock);
     for (size_t i = 0; i < gInstances.size (); i++)
@@ -1349,9 +1372,7 @@ int mb200_set_tip_states (int instance, int tip, const uint64_t *masks)
     if (tip < 0 || tip >= I->cfg.tip_count || !masks) return MB200_ERROR_OUT_OF_RANGE;
     int rc = use (I); if (rc) return rc;
     const int C = I->cfg.pattern_count;
-    rc = ensureStage (I, (size_t)C * 9); if (rc) return rc;
-    uint64_t *h64 = (uint64_t *) I->hostStage;
-    uint8_t  *h8  = (uint8_t *)(h64 + C);
+    std::vector<uint64_t> h64 (C); std::vector<uint8_t> h8 (C);     // pageable: the copies are waited for below
     const uint64_t full = (I->cfg.state_count == 64) ? ~(uint64_t)0 : (((uint64_t)1 << I->cfg.state_count) - 1);
     int partAmbig = 0;      // isPartAmbig of SetUpTermState (src/mcmc.c:18631-18651)
     for (int c = 0; c < C; c++)
@@ -1364,8 +1385,8 @@ int mb200_set_tip_states (int instance, int tip, const uint64_t *masks)
     CK (cudaMemcpyAsync (I->dTipPartAmbig + tip, &partAmbig, sizeof(int), cudaMemcpyHostToDevice, I->stream));
     I->tipPartAmbig[tip] = partAmbig;
     I->tipEpoch++;                  // packed 4-state batches carry the tip kinds: re-pack after this
-    CK (cudaMemcpyAsync (I->dTip64 + (size_t)tip * C, h64, (size_t)C * 8, cudaMemcpyHostToDevice, I->stream));
-    CK (cudaMemcpyAsync (I->dTip8 + (size_t)tip * C, h8, (size_t)C, cudaMemcpyHostToDevice, I->stream));
+    CK (cudaMemcpyAsync (I->dTip64 + (size_t)tip * C, h64.data (), (size_t)C * 8, cudaMemcpyHostToDevice, I->stream));
+    CK (cudaMemcpyAsync (I->dTip8 + (size_t)tip * C, h8.data (), (size_t)C, cudaMemcpyHostToDevice, I->stream));
     CK (cudaStreamSynchronize (I->stream));
     I->invMaskValid = false;
     return MB200_SUCCESS;
@@ -1407,22 +1428,23 @@ int mb200_set_pattern_states (int instance, const int *ns, const int *ti, const 
             classes.push_back (make_int2 (ns[c], ti[c]));
             }
         }
+    // the new tables and matrices (a branch's: one block of matLen floats, m->tiProbLength) are complete before the
+    // old ones go: on failure the instance keeps those
+    const size_t matFloats = (size_t)I->cfg.matrix_count * matLen;
+    DevArray<int> dTab; DevArray<int2> dClasses; DevArray<float> dMats;
+    if ((rc = dTab.alloc (3 * (size_t)C)) || (rc = dClasses.alloc (MB200_STD_MAX_STATES)) || (rc = dMats.alloc (matFloats))) return rc;
+    CK (cudaMemsetAsync (dMats, 0, matFloats * sizeof(float), I->stream));
+    CK (cudaMemcpyAsync (dTab, ns, (size_t)C * sizeof(int), cudaMemcpyHostToDevice, I->stream));
+    CK (cudaMemcpyAsync (dTab + C, ti, (size_t)C * sizeof(int), cudaMemcpyHostToDevice, I->stream));
+    CK (cudaMemcpyAsync (dTab + 2*(size_t)C, bs, (size_t)C * sizeof(int), cudaMemcpyHostToDevice, I->stream));
+    CK (cudaMemcpyAsync (dClasses, classes.data (), classes.size () * sizeof(int2), cudaMemcpyHostToDevice, I->stream));
+    CK (cudaStreamSynchronize (I->stream));
+    I->dStdTab = std::move (dTab); I->dStdClasses = std::move (dClasses); I->dMatrices = std::move (dMats);
+    I->ctx.matrices = I->dMatrices;
+    I->ring = MatRing ();                       // its slots hold matrices of the old length
     I->hNStates.assign (ns, ns + C); I->hTiIndex.assign (ti, ti + C); I->hBsIndex.assign (bs, bs + C);
     I->hClOff.assign (C + 1, 0);
     for (int c = 0; c < C; c++) I->hClOff[c + 1] = I->hClOff[c] + (size_t) ns[c];
-    std::vector<int> tab (3 * (size_t)C);
-    memcpy (tab.data (), ns, (size_t)C * sizeof(int));
-    memcpy (tab.data () + C, ti, (size_t)C * sizeof(int));
-    memcpy (tab.data () + 2*(size_t)C, bs, (size_t)C * sizeof(int));
-    CK (cudaStreamSynchronize (I->stream));
-    // a branch's matrices are one block of matLen floats (m->tiProbLength)
-    cudaFree (I->dMatrices); I->dMatrices = nullptr;
-    CK (cudaMalloc ((void **)&I->dMatrices, (size_t)I->cfg.matrix_count * matLen * sizeof(float)));
-    CK (cudaMemsetAsync (I->dMatrices, 0, (size_t)I->cfg.matrix_count * matLen * sizeof(float), I->stream));
-    I->ctx.matrices = I->dMatrices;
-    CK (cudaMemcpyAsync (I->dStdTab, tab.data (), tab.size () * sizeof(int), cudaMemcpyHostToDevice, I->stream));
-    CK (cudaMemcpyAsync (I->dStdClasses, classes.data (), classes.size () * sizeof(int2), cudaMemcpyHostToDevice, I->stream));
-    CK (cudaStreamSynchronize (I->stream));
     I->sx.nStates = I->dStdTab; I->sx.tiIndex = I->dStdTab + C; I->sx.bsIndex = I->dStdTab + 2*(size_t)C;
     I->sx.classes = I->dStdClasses; I->sx.nClasses = (int) classes.size ();
     I->sx.matLen = matLen; I->sx.dummy = dummy; I->sx.uncompressed = uncompressed;
@@ -1437,7 +1459,7 @@ int mb200_set_cijk (int instance, int eigen, const double *block)
     if (!I) return MB200_ERROR_BAD_INSTANCE;
     if (eigen < 0 || eigen >= I->cfg.eigen_count || !block) return MB200_ERROR_OUT_OF_RANGE;
     int rc = use (I); if (rc) return rc;
-    if (!I->eigWarmChain.empty ()) I->eigWarmChain[eigen] = -1;        // this slot's eigenvectors no longer come from the device solver
+    if (!I->eig.warmChain.empty ()) I->eig.warmChain[eigen] = -1;      // this slot's eigenvectors no longer come from the device solver
     CK (cudaMemcpyAsync (I->dEigen + (size_t)eigen * I->eigenStride, block, I->eigenStride * sizeof(double),
                          cudaMemcpyHostToDevice, I->stream));
     if (I->dFactor)
@@ -1459,26 +1481,24 @@ int mb200_set_eigen_decomposition (int instance, int eigen, const double *V, con
     if (eigen < 0 || eigen >= I->cfg.eigen_count || !V || !Vinv || !lambda) return MB200_ERROR_OUT_OF_RANGE;
     if (I->cijkParts != 1) return MB200_ERROR_UNSUPPORTED;        // multi-part slots are uploaded whole (mb200_set_cijk)
     int rc = use (I); if (rc) return rc;
-    if (!I->eigWarmChain.empty ()) I->eigWarmChain[eigen] = -1;
+    if (!I->eig.warmChain.empty ()) I->eig.warmChain[eigen] = -1;
     const int S = I->cfg.state_count;
     const size_t n2 = (size_t)S * S;
-    double *tmp = nullptr;
-    CK (cudaMalloc ((void **)&tmp, (2*n2 + S) * sizeof(double)));
-    cudaMemcpyAsync (tmp, V, n2 * sizeof(double), cudaMemcpyHostToDevice, I->stream);
-    cudaMemcpyAsync (tmp + n2, Vinv, n2 * sizeof(double), cudaMemcpyHostToDevice, I->stream);
-    cudaMemcpyAsync (tmp + 2*n2, lambda, (size_t)S * sizeof(double), cudaMemcpyHostToDevice, I->stream);
+    DevArray<double> tmp;                   // freed on return, after the stream has been waited for
+    if ((rc = tmp.alloc (2*n2 + S))) return rc;
+    CK (cudaMemcpyAsync (tmp, V, n2 * sizeof(double), cudaMemcpyHostToDevice, I->stream));
+    CK (cudaMemcpyAsync (tmp + n2, Vinv, n2 * sizeof(double), cudaMemcpyHostToDevice, I->stream));
+    CK (cudaMemcpyAsync (tmp + 2*n2, lambda, (size_t)S * sizeof(double), cudaMemcpyHostToDevice, I->stream));
     size_t n3 = n2 * S;
     int blocks = (int)((n3 + 255) / 256); if (blocks > 1024) blocks = 1024;
     cijk_kernel<<<blocks, 256, 0, I->stream>>> (I->dEigen + (size_t)eigen * I->eigenStride, tmp, tmp + n2, tmp + 2*n2, S);
     I->launchKind[MB200_KERNEL_SETUP]++;
     if (I->dFactor)         // the factors are the caller's V and V^-1 themselves
         {
-        cudaMemcpyAsync (I->dFactor + (size_t)eigen * 2 * n2, tmp, n2 * sizeof(double), cudaMemcpyDeviceToDevice, I->stream);
-        cudaMemcpyAsync (I->dFactor + (size_t)eigen * 2 * n2 + n2, tmp + n2, n2 * sizeof(double), cudaMemcpyDeviceToDevice, I->stream);
+        CK (cudaMemcpyAsync (I->dFactor + (size_t)eigen * 2 * n2, tmp, n2 * sizeof(double), cudaMemcpyDeviceToDevice, I->stream));
+        CK (cudaMemcpyAsync (I->dFactor + (size_t)eigen * 2 * n2 + n2, tmp + n2, n2 * sizeof(double), cudaMemcpyDeviceToDevice, I->stream));
         }
-    cudaError_t e = cudaStreamSynchronize (I->stream);
-    cudaFree (tmp);
-    CK (e);
+    CK (cudaStreamSynchronize (I->stream));
     return MB200_SUCCESS;
 }
 
@@ -1496,46 +1516,27 @@ int mb200_set_rate_matrices (int instance, int eigen, int like_eigen, const doub
     const size_t n2 = (size_t)S * S;
     const int    N = (S + 1) & ~1;
     const size_t uLen = (size_t)parts * N * N;
-    if (!I->dEigIn)
-        {
-        I->eigInStride = (size_t)parts * n2 + S;
-        const size_t bytes = (size_t)I->cfg.eigen_count * I->eigInStride * sizeof(double);
-        CK (cudaMalloc ((void **)&I->dEigIn, bytes));
-        CK (cudaHostAlloc ((void **)&I->hEigIn, bytes, cudaHostAllocDefault));
-        CK (cudaHostAlloc ((void **)&I->hEigStatus, sizeof(int), cudaHostAllocMapped));
-        *I->hEigStatus = 0;
-        if (I->dFactor) I->dEigVec = I->dFactor;
-        else CK (cudaMalloc ((void **)&I->dEigVec, (size_t)I->cfg.eigen_count * parts * 2 * n2 * sizeof(double)));
-        CK (cudaMalloc ((void **)&I->dEigU, (size_t)I->cfg.eigen_count * uLen * sizeof(double)));
-        CK (cudaMalloc ((void **)&I->dEigLog, (size_t)parts * MB200_EIG_LOG_DOUBLES * sizeof(double)));
-        CK (cudaMalloc ((void **)&I->dEigRounds, (size_t)parts * sizeof(int)));
-        I->eigWarmChain.assign (I->cfg.eigen_count, -1);
-        I->evEigIn.resize (I->cfg.eigen_count);
-        for (auto &e : I->evEigIn) CK (cudaEventCreateWithFlags (&e, cudaEventDisableTiming));
-        CK (cudaFuncSetAttribute (eigen_rotations_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) eigen_smem_bytes ()));
-        }
-    else
-        CK (cudaEventSynchronize (I->evEigIn[eigen]));                 // the slot's previous matrices have left the staging area
-    double *h = I->hEigIn + (size_t)eigen * I->eigInStride, *d = I->dEigIn + (size_t)eigen * I->eigInStride;
+    if (!I->eig.dIn && (rc = makeEigenSolver (I, I->eig))) return rc;
+    EigenSolver &g = I->eig;
+    CK (cudaEventSynchronize (g.evIn[eigen]));              // the slot's previous matrices have left the staging area
+    double *h = g.hIn + (size_t)eigen * g.inStride, *d = g.dIn + (size_t)eigen * g.inStride;
     memcpy (h, Q, (size_t)parts * n2 * sizeof(double));
     memcpy (h + (size_t)parts * n2, pi, (size_t)S * sizeof(double));
-    CK (cudaMemcpyAsync (d, h, I->eigInStride * sizeof(double), cudaMemcpyHostToDevice, I->stream));
-    CK (cudaEventRecord (I->evEigIn[eigen], I->stream));
-    int *dStatus = nullptr;
-    CK (cudaHostGetDevicePointer ((void **)&dStatus, I->hEigStatus, 0));
+    CK (cudaMemcpyAsync (d, h, g.inStride * sizeof(double), cudaMemcpyHostToDevice, I->stream));
+    CK (cudaEventRecord (g.evIn[eigen], I->stream));
     // warm start from the eigenvectors of a nearby matrix, unless that would extend an already long chain of warm starts
     const double *U0 = nullptr;
     int chain = 0;
-    if (like_eigen >= 0 && like_eigen != eigen && I->eigWarmChain[like_eigen] >= 0 && I->eigWarmChain[like_eigen] < MB200_EIG_WARM_CHAIN)
+    if (like_eigen >= 0 && like_eigen != eigen && g.warmChain[like_eigen] >= 0 && g.warmChain[like_eigen] < MB200_EIG_WARM_CHAIN)
         {
-        U0 = I->dEigU + (size_t)like_eigen * uLen;
-        chain = I->eigWarmChain[like_eigen] + 1;
+        U0 = g.U + (size_t)like_eigen * uLen;
+        chain = g.warmChain[like_eigen] + 1;
         }
-    I->eigWarmChain[eigen] = chain;
+    g.warmChain[eigen] = chain;
     const double *dPi = d + (size_t)parts * n2;
-    double *vec = I->dEigVec + (size_t)eigen * parts * 2 * n2, *block = I->dEigen + (size_t)eigen * I->eigenStride;
-    eigen_rotations_kernel<<<parts, MB200_EIG_THREADS, eigen_smem_bytes (), I->stream>>> (d, dPi, S, U0, I->dEigLog, I->dEigRounds, block, dStatus);
-    eigen_vectors_kernel<<<dim3 ((N + 7) / 8, parts), 256, 0, I->stream>>> (dPi, S, U0, I->dEigLog, I->dEigRounds, I->dEigU + (size_t)eigen * uLen, vec);
+    double *vec = (I->dFactor ? I->dFactor : g.vec) + (size_t)eigen * parts * 2 * n2, *block = I->dEigen + (size_t)eigen * I->eigenStride;
+    eigen_rotations_kernel<<<parts, MB200_EIG_THREADS, eigen_smem_bytes (), I->stream>>> (d, dPi, S, U0, g.log, g.rounds, block, g.status.dev);
+    eigen_vectors_kernel<<<dim3 ((N + 7) / 8, parts), 256, 0, I->stream>>> (dPi, S, U0, g.log, g.rounds, g.U + (size_t)eigen * uLen, vec);
     const size_t n3 = n2 * S;
     int blocks = (int)((n3 + 255) / 256); if (blocks > 512) blocks = 512;
     cijk_parts_kernel<<<dim3 (blocks, parts), 256, 0, I->stream>>> (block, vec, S);
@@ -1733,19 +1734,19 @@ int mb200_set_transition_matrix (int instance, int matrix, const float *in)
         {
         // small matrices (host-built P(t) of a STANDARD division, one call per dirty branch): stage through a pinned ring and let
         // the copy ride the instance's stream -- the evaluation that reads the matrix is queued behind it; no host wait
-        if (!I->hMatRing)
+        if (I->ring.stride < n)                                 // none yet (mb200_set_pattern_states drops it)
             {
-            I->matRingStride = n;
-            CK (cudaHostAlloc ((void **)&I->hMatRing, (size_t)MAT_RING * n * sizeof(float), cudaHostAllocDefault));
-            I->evMatRing.resize (MAT_RING);
-            for (auto &e : I->evMatRing) CK (cudaEventCreateWithFlags (&e, cudaEventDisableTiming));
+            MatRing r;
+            if ((rc = r.buf.alloc ((size_t)MAT_RING * n)) || (rc = makeEvents (r.ev, MAT_RING, cudaEventDisableTiming))) return rc;
+            r.stride = n;
+            I->ring = std::move (r);
             }
-        const int slot = I->matRingNext++ % MAT_RING;
-        CK (cudaEventSynchronize (I->evMatRing[slot]));           // the slot's previous copy has left the ring
-        float *h = I->hMatRing + (size_t)slot * I->matRingStride;
+        const int slot = I->ring.next++ % MAT_RING;
+        CK (cudaEventSynchronize (I->ring.ev[slot]));           // the slot's previous copy has left the ring
+        float *h = I->ring.buf + (size_t)slot * I->ring.stride;
         memcpy (h, in, n * sizeof(float));
         CK (cudaMemcpyAsync (I->dMatrices + (size_t)matrix * n, h, n * sizeof(float), cudaMemcpyHostToDevice, I->stream));
-        CK (cudaEventRecord (I->evMatRing[slot], I->stream));
+        CK (cudaEventRecord (I->ring.ev[slot], I->stream));
         return MB200_SUCCESS;
         }
     CK (cudaMemcpyAsync (I->dMatrices + (size_t)matrix * n, in, n * sizeof(float), cudaMemcpyHostToDevice, I->stream));
@@ -1793,16 +1794,17 @@ int mb200_pack_evaluations (int instance, const mb200_evaluation *evaluations, i
     if (!I) return MB200_ERROR_BAD_INSTANCE;
     if (!evaluations || !batch) return MB200_ERROR_OUT_OF_RANGE;
     int rc = use (I); if (rc) return rc;
-    Batch *b = new Batch ();
+    auto b = std::make_unique<Batch> ();
     rc = pack (I, *b, evaluations, count);
-    if (rc != MB200_SUCCESS) { freeBatch (*b); delete b; return rc; }
+    if (rc != MB200_SUCCESS) return rc;
     if (cudaMemcpyAsync (b->dBlob, b->hBlob, b->bytes, cudaMemcpyHostToDevice, I->stream) != cudaSuccess ||
         cudaStreamSynchronize (I->stream) != cudaSuccess)
-        { freeBatch (*b); delete b; return MB200_ERROR_CUDA; }
-    for (size_t i = 0; i < I->batches.size (); i++)
-        if (I->batches[i] == nullptr) { I->batches[i] = b; *batch = (int) i; return MB200_SUCCESS; }
-    I->batches.push_back (b);
-    *batch = (int) I->batches.size () - 1;
+        return MB200_ERROR_CUDA;
+    size_t i = 0;
+    while (i < I->batches.size () && I->batches[i]) i++;
+    if (i == I->batches.size ()) I->batches.emplace_back ();
+    I->batches[i] = std::move (b);
+    *batch = (int) i;
     return MB200_SUCCESS;
 }
 
@@ -1866,11 +1868,11 @@ int mb200_free_batch (int instance, int batch)
     Instance *I = get (instance);
     if (!I) return MB200_ERROR_BAD_INSTANCE;
     if (batch < 0 || batch >= (int) I->batches.size () || !I->batches[batch]) return MB200_ERROR_OUT_OF_RANGE;
+    if (I->pending.count > 0 && I->pending.batch == I->batches[batch].get ())
+        return MB200_ERROR_OUT_OF_RANGE;          // the pending evaluation writes its results there
     int rc = use (I); if (rc) return rc;
     CK (cudaStreamSynchronize (I->stream));
-    freeBatch (*I->batches[batch]);
-    delete I->batches[batch];
-    I->batches[batch] = nullptr;
+    I->batches[batch].reset ();
     return MB200_SUCCESS;
 }
 
@@ -1917,12 +1919,9 @@ int mb200_set_kernel_timing (int instance, int enabled)
     CK (cudaStreamSynchronize (I->stream));
     if (enabled && I->evA.empty ())
         {
-        I->evA.resize (EV_RING); I->evB.resize (EV_RING);
-        for (int i = 0; i < EV_RING; i++)
-            {
-            CK (cudaEventCreate (&I->evA[i]));
-            CK (cudaEventCreate (&I->evB[i]));
-            }
+        std::vector<Event> a, b;
+        if ((rc = makeEvents (a, EV_RING, cudaEventDefault)) || (rc = makeEvents (b, EV_RING, cudaEventDefault))) return rc;
+        I->evA = std::move (a); I->evB = std::move (b);
         }
     I->timing = enabled != 0;
     I->evCount = 0;
