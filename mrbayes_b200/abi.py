@@ -134,6 +134,8 @@ class Library:
             "pack_evaluations": [I, P(Evaluation), I, P(I)],
             "replay": [I, I],
             "replay_results": [I, I, P(D), P(I)],
+            "replay_begin": [I, I],
+            "replay_end": [I, P(D), P(I)],
             "free_batch": [I, I],
             "synchronize": [I],
             "get_stream": [I, P(C.c_void_p)],
@@ -255,6 +257,7 @@ class Instance:
         self.variable_states = bool(flags & CONFIG_VARIABLE_STATES)
         self.state_counts = None
         self.matrix_length = None
+        self.batch_sizes = {}           # packed batch -> its evaluation count
 
     # -- lifetime --------------------------------------------------------------------
     def close(self):
@@ -276,6 +279,13 @@ class Instance:
 
     def _call(self, name, *args):
         self.lib.check(name, self.lib.fn(name)(self.handle, *args))
+
+    def _results(self, name, n, *args):
+        """name(handle, *args, lnL, status) with room for n results -> (lnL, status)"""
+        lnl = np.zeros(n, np.float64)
+        st = np.zeros(n, np.int32)
+        self._call(name, *args, _ptr(lnl, C.c_double), _ptr(st, C.c_int))
+        return lnl, st
 
     # -- static data -------------------------------------------------------------------
     def set_tip_states(self, tip: int, masks):
@@ -324,12 +334,7 @@ class Instance:
     def evaluate(self, specs):
         if isinstance(specs, EvalSpec):
             specs = [specs]
-        arr = make_eval_array(specs)
-        n = len(specs)
-        lnl = np.zeros(n, np.float64)
-        st = np.zeros(n, np.int32)
-        self._call("evaluate", arr, n, _ptr(lnl, C.c_double), _ptr(st, C.c_int))
-        return lnl, st
+        return self._results("evaluate", len(specs), make_eval_array(specs), len(specs))
 
     def evaluate_begin(self, specs):
         """First half of evaluate(): validate, pack, launch; returns at once (one in flight per instance)."""
@@ -340,27 +345,31 @@ class Instance:
         self._call("evaluate_begin", self._pending, self._pending_n)
 
     def evaluate_end(self):
-        n = self._pending_n
-        lnl = np.zeros(n, np.float64)
-        st = np.zeros(n, np.int32)
-        self._call("evaluate_end", _ptr(lnl, C.c_double), _ptr(st, C.c_int))
+        out = self._results("evaluate_end", self._pending_n)
         self._pending = None
-        return lnl, st
+        return out
 
     def pack(self, specs) -> int:
         arr = make_eval_array(specs)
         b = C.c_int(-1)
         self._call("pack_evaluations", arr, len(specs), C.byref(b))
+        self.batch_sizes[b.value] = len(specs)
         return b.value
 
     def replay(self, batch: int):
         self._call("replay", batch)
 
     def replay_results(self, batch: int, n: int):
-        lnl = np.zeros(n, np.float64)
-        st = np.zeros(n, np.int32)
-        self._call("replay_results", batch, _ptr(lnl, C.c_double), _ptr(st, C.c_int))
-        return lnl, st
+        return self._results("replay_results", n, batch)
+
+    def replay_begin(self, batch: int):
+        """First half of replaying a packed batch, on the resident kernel when the engine admits it there;
+        replay_end() collects the results (one evaluation in flight per instance)."""
+        self._call("replay_begin", batch)
+        self._pending_n = self.batch_sizes[batch]
+
+    def replay_end(self):
+        return self._results("replay_end", self._pending_n)
 
     def free_batch(self, batch: int):
         self._call("free_batch", batch)
@@ -429,6 +438,12 @@ class Instance:
         out = np.zeros((self.K, self.C, self.S), np.float32)
         self._call("get_partials", buffer, _ptr(out, C.c_float))
         return out
+
+    def set_transition_matrix(self, matrix: int, block):
+        """A caller-supplied P(t): [K, S, S] floats, or for variable-state divisions a block of matrix_length"""
+        b = np.ascontiguousarray(block, np.float32)
+        assert b.size == (self.matrix_length if self.variable_states else self.K * self.S * self.S)
+        self._call("set_transition_matrix", matrix, _ptr(b, C.c_float))
 
     def set_partials(self, buffer: int, a):
         a = np.ascontiguousarray(a, np.float32)

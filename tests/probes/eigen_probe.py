@@ -5,16 +5,16 @@ from pathlib import Path
 import numpy as np
 HERE = Path(__file__).resolve().parent
 sys.path.insert(0, str(HERE.parents[1]))         # the repository: mrbayes_b200
-sys.path.insert(0, str(HERE.parent))             # tests/: test_gpu_eigen
+sys.path.insert(0, str(HERE.parent))             # tests/: engine_checks
+from engine_checks import eigen_instance, reversible_q
 from mrbayes_b200 import abi
-from test_gpu_eigen import reversible_q, make
 
 lib = abi.engine_library()
 for S, K, parts in [(4, 4, 1), (20, 4, 1), (61, 1, 1), (61, 3, 3), (64, 1, 1)]:
     rng = np.random.default_rng(S)
     Q, pi = reversible_q(rng, S, sparse=(S > 20))
     Qs = np.stack([Q * (1 + 0.3 * p) for p in range(parts)])
-    with make(lib, S, K, parts) as dev:
+    with eigen_instance(lib, S, K, parts) as dev:
         for _ in range(5):
             dev.set_rate_matrices(0, Qs, pi)
         dev._call("synchronize")
@@ -31,7 +31,7 @@ for S, K, parts in [(4, 4, 1), (20, 4, 1), (61, 1, 1), (61, 3, 3), (64, 1, 1)]:
 for S, K, parts in [(61, 1, 1), (61, 3, 3), (20, 4, 1)]:
     rng = np.random.default_rng(S)
     Q, pi = reversible_q(rng, S, sparse=(S > 20))
-    with make(lib, S, K, parts) as dev:
+    with eigen_instance(lib, S, K, parts) as dev:
         dev.set_rate_matrices(0, np.stack([Q] * parts), pi)
         n = 60
         Qs = []

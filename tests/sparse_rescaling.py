@@ -11,11 +11,15 @@ Per chain, a table counts the unscaled interior levels below each node (tips cou
 
 A copy of the table is kept with each evaluation and put back when it is rejected
 (unscaledNodesScratch, src/likelihood.c:5645).  f = 1 gives Problem's own lists; f = inf never
-rescales."""
+rescales.
+
+The threshold_* builders at the end set up one-node evaluations whose rescaler maximum or root
+likelihood sits exactly at the float-range guard's threshold (MB200_FLAG_RANGE_GUARD)."""
 import types
 
 import numpy as np
 
+from engine_checks import num_sms, ppb, resident_generations, via_evaluate, via_replay
 from mrbayes_b200 import abi, workloads
 
 
@@ -90,3 +94,65 @@ def unscaled_maxima(pr, ch):
         cl[p] = x
         out[p] = x.max(axis=(0, 2))
     return out
+
+
+# ---- the float-range guard at its threshold -------------------------------------------------------------------------
+GUARD_MIN = np.float32(1e-24)
+THRESHOLD_C = {"host": 10, "device": 40, "non_fused": None, "throughput": 10, "resident": 12}   # resident: <= 16 tiles
+
+
+def threshold_setup(route, K, where, n_eval):
+    """n_eval evaluations of one node each over 4 tips (buffers and slots of chain e for evaluation e):
+    the node multiplies interior buffers x and 1.0 through P = I (branch length 0).  -> problem, C,
+    the pattern that will carry the value"""
+    tiles = THRESHOLD_C[route] or 4 * num_sms() + 4
+    C = tiles * ppb(K) - (ppb(K) - 1 if where == "last" else 0)
+    pr = workloads.make_problem(4, K, C, 4, n_eval, seed=12, flags=abi.FLAG_NUC4_PINVAR_QUIRK | abi.FLAG_RANGE_GUARD)
+    pr.freqs = np.full(4, 0.25)
+    return pr, C, (C - 1 if where == "last" else C // 2 + 1)
+
+
+def threshold_spec(pr, e_idx, kind):
+    """kind 'node': buffer a -> rescaled node d1 -> unscaled root d2; kind 'root': a -> unscaled root d1"""
+    nI = pr.n_int
+    a, ones, d1, d2 = (pr.n_tips + 2 * e_idx * nI + j for j in range(4))
+    mat = 2 * e_idx * pr.n_nodes
+    base = 2 * e_idx * (nI + 1)
+    op = lambda dest, c1, sw: (dest, c1, mat, ones, mat, abi.NONE, abi.NONE, sw, abi.NONE)
+    ops = [op(d1, a, base), op(d2, d1, abi.NONE)] if kind == "node" else [op(d1, a, abi.NONE)]
+    return abi.EvalSpec(mats=np.array([(mat, 0, 0.0)], abi.MAT_DTYPE), ops=np.array(ops, abi.OP_DTYPE),
+                        site_dst=base + 1, site_src=abi.NONE, root=ops[-1][0], flags=pr.flags,
+                        rates=pr.rates, cat_weights=np.full(pr.K, 1.0 / pr.K), freqs=pr.freqs, chain=e_idx)
+
+
+def threshold_partials(pr, kind, c, x):
+    """'node': 0.5 everywhere but x at pattern c -- its maximum; 'root' (K = 1, frequencies 1/4):
+    1.0 everywhere but x in every state of c, so that likeF = 4 (x / 4) = x exactly"""
+    a = np.full((pr.K, pr.C, 4), 0.5 if kind == "node" else 1.0, np.float32)
+    if x is not None:
+        a[:, c, :] = x
+    return a
+
+
+def run_threshold(e, o, route, gens):
+    """each generation (a list of evaluations) on the route and on the oracle -> [(lnL, status, oracle
+    lnL, oracle status)] per evaluation, per generation.  The resident route packs every generation
+    first, so that one kernel can serve them all."""
+    if route == "resident":
+        got = resident_generations(e, gens)
+    else:
+        got = [(via_replay if route == "device" else via_evaluate)(e, specs) for specs in gens]
+    out = []
+    for (lnl, st), specs in zip(got, gens):
+        out.append([(lnl[i], st[i]) + tuple(x[0] for x in o.evaluate(sp)) for i, sp in enumerate(specs)])
+    return out
+
+
+def threshold_instance(pr, lib, route, values, kind, c):
+    e = pr.create(lib, flags=abi.CONFIG_THROUGHPUT if route == "throughput" else 0)
+    ones = np.ones((pr.K, pr.C, 4), np.float32)
+    for i, x in enumerate(values):
+        base = pr.n_tips + 2 * i * pr.n_int
+        e.set_partials(base, threshold_partials(pr, kind, c, x))
+        e.set_partials(base + 1, ones)
+    return e

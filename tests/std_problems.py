@@ -171,8 +171,7 @@ class MatrixSupplier:
             blk = np.ascontiguousarray(self.make(pr, ch, node), np.float32)
             self.blocks[ch, int(mu["matrix"])] = blk
             for inst in insts:
-                inst.lib.check("set_transition_matrix", inst.lib.fn("set_transition_matrix")(
-                    inst.handle, int(mu["matrix"]), blk.ctypes.data_as(abi.C.POINTER(abi.C.c_float))))
+                inst.set_transition_matrix(int(mu["matrix"]), blk)
         sp.mats = sp.mats[keep].copy()
         return sp
 
@@ -180,23 +179,6 @@ class MatrixSupplier:
         """node -> the block the instances hold for chain ch's current matrix of that branch"""
         ti = self.pr.chains[ch].ti
         return {node: self.blocks[ch, int(ti[node])] for node in self.nodes(ch) if (ch, int(ti[node])) in self.blocks}
-
-
-def run_specs(pr, updates, seed):
-    """A full evaluation per chain, then `updates` branch updates over the chains in turn; every third update is
-    rejected once the caller has evaluated it.  Yields the evaluations."""
-    rng = np.random.default_rng(seed)
-    for ch in range(pr.n_chains):
-        yield pr.full_evaluation(ch)
-    for it in range(updates):
-        ch = it % pr.n_chains
-        old = pr.tree[ch].length.copy()
-        sp = pr.random_branch_update(ch, rng)
-        mats = sp.mats.copy()                            # a MatrixSupplier takes its updates out of sp
-        yield sp
-        if it % 3 == 2:
-            sp.mats = mats                               # every branch whose matrix index flipped flips back
-            pr.reject(ch, sp, old)
 
 
 # ----------------------------------------------------------------------------- the shapes the Std tests run

@@ -154,12 +154,13 @@ def test_f64_reference_matrix_exponential_matches_eigensystem():
 # ---- variable-state (Std) divisions: the float64 reference against the oracle at the shapes of test_gpu_std.py ----
 def std_oracle_run(oracle_lib, name, updates=6):
     """-> [(evaluation, oracle lnL, oracle status, float64 StdLnl)] of a full evaluation per chain and branch updates"""
+    from engine_checks import evaluation_sequence
     from f64_reference import f64_std_lnl
-    from std_problems import make_case, run_specs
+    from std_problems import make_case
     pr, supplier = make_case(name)
     out = []
     with pr.create(oracle_lib) as o:
-        for sp in run_specs(pr, updates, seed=1):
+        for _, sp in evaluation_sequence(pr, updates, seed=1):
             if supplier:
                 supplier(sp, [o])
             (lo,), (so,) = o.evaluate(sp)

@@ -20,15 +20,13 @@ import numpy as np
 import pytest
 
 from chain_models import MixedModels
+from engine_checks import (DBL_MAX, SYN_RTOL, check_with_oracle, compare_written, edge, lnl_tol, num_sms, ppb, rel,
+                           resident_generations, tree_tol, via_evaluate, via_replay)
 from f64_reference import caterpillar_tree, transition_matrices
 from mrbayes_b200 import abi, workloads
-from test_gpu_parity import SYN_RTOL, rel
-from test_gpu_paths import compare_state, edge, num_sms, ppb, tol_of, via_evaluate, via_replay
-from test_gpu_rescaling import GUARD_MIN, run_threshold, threshold_instance, threshold_setup, threshold_spec
+from sparse_rescaling import GUARD_MIN, run_threshold, threshold_instance, threshold_setup, threshold_spec
 
 pytestmark = pytest.mark.gpu
-
-DBL_MAX = np.finfo(np.float64).max
 ROLES = ["upd", "root", "upd", "nomat", "upd", "full"]
 
 
@@ -61,14 +59,6 @@ def batch(mm, g, rng, counts, full=()):
     return specs, rejects
 
 
-def check_against_oracle(mm, e, o, specs, lnl, st, tol):
-    for i, sp in enumerate(specs):
-        (lo,), (so,) = o.evaluate(sp)
-        assert st[i] == so == abi.EVAL_OK, f"evaluation {i} (chain {sp.chain})"
-        assert rel(lnl[i], lo) < tol, f"evaluation {i} (chain {sp.chain}): {rel(lnl[i], lo):.2e}"
-        compare_state(e, o, sp, mm.pr)
-
-
 def check_against_f64(mm, specs, lnl, tol):
     if mm.std:
         return
@@ -88,7 +78,7 @@ def check_alone(got, lnl, bitwise, tol):
 
 def mixed_run(mm, e, o, twin, oracle_lib, route, bitwise, gens=5, seed=0):
     """gens mixed batches on `route`, then the permutation check -> number of calls made on e"""
-    pr, tol = mm.pr, tol_of(mm.pr.S)
+    pr, tol = mm.pr, lnl_tol(mm.pr.S)
     n = pr.n_chains
     with mm.create(oracle_lib) as scratch:
         scratch.set_arith(1)
@@ -99,7 +89,7 @@ def mixed_run(mm, e, o, twin, oracle_lib, route, bitwise, gens=5, seed=0):
         specs, rejects = batch(mm, g, rng, counts)
         lnl, st = route(e, specs)
         check_alone([twin.evaluate(sp) for sp in specs], lnl, bitwise, tol)
-        check_against_oracle(mm, e, o, specs, lnl, st, tol)
+        check_with_oracle(e, o, specs, lnl, st, tol, tree_tol(pr))
         if g in (0, gens - 1):
             check_against_f64(mm, specs, lnl, tol)
         for ch, sp, old in rejects:
@@ -212,20 +202,6 @@ def test_std(engine_lib, oracle_lib):
 
 
 # ---- resident ---------------------------------------------------------------------------------------------------------
-def replay_resident(lib, e, batches, n, before=None):
-    out = []
-    for g, b in enumerate(batches):
-        if before:
-            before(g, e)
-        lnl = np.zeros(n, np.float64)
-        st = np.zeros(n, np.int32)
-        assert lib.fn("replay_begin")(e.handle, b) == 0
-        assert lib.fn("replay_end")(e.handle, lnl.ctypes.data_as(abi.C.POINTER(abi.C.c_double)),
-                                    st.ctypes.data_as(abi.C.POINTER(abi.C.c_int))) == 0
-        out.append((lnl, st))
-    return out
-
-
 @pytest.mark.parametrize("K", [2, 4, 5])
 def test_nuc4_resident(engine_lib, oracle_lib, K):
     """replay_begin / _end with the instance alone on the device.  Generation g gives chain ch weights row
@@ -276,26 +252,24 @@ def test_nuc4_resident(engine_lib, oracle_lib, K):
         mm.assert_models_differ(scratch, range(n))
     with mm.create(engine_lib) as e, mm.create(oracle_lib) as o:
         o.set_arith(1)
-        batches = [e.pack(specs) for specs in gens]
         n0 = e.kernel_launches(abi.KERNEL_NUC4)
-        got = replay_resident(engine_lib, e, batches, n, set_calls)
+        got = resident_generations(e, gens, set_calls)
         launches = e.kernel_launches(abi.KERNEL_NUC4) - n0
         e.synchronize()
         assert launches <= G // 2          # one kernel served several generations (the set calls retire it)
         for g, specs in enumerate(gens):
             set_calls(g, o)
             lnl, st = got[g]
-            for i, sp in enumerate(specs):
-                (lo,), (so,) = o.evaluate(sp)
-                assert st[i] == so == abi.EVAL_OK, f"generation {g}, evaluation {i}"
-                assert rel(lnl[i], lo) < SYN_RTOL, f"generation {g}, evaluation {i}: {rel(lnl[i], lo):.2e}"
+            if g == G - 1:                 # the engine holds the last generation's buffers: compare them too
+                check_with_oracle(e, o, specs, lnl, st, SYN_RTOL, tree_tol(mm.pr))
+            else:
+                for i, sp in enumerate(specs):
+                    (lo,), (so,) = o.evaluate(sp)
+                    assert st[i] == so == abi.EVAL_OK, f"generation {g}, evaluation {i}"
+                    assert rel(lnl[i], lo) < SYN_RTOL, f"generation {g}, evaluation {i}: {rel(lnl[i], lo):.2e}"
             if g in expect:
                 for i, want in enumerate(expect[g]):
                     assert rel(lnl[i], want) < SYN_RTOL, f"float64 reference, generation {g}, evaluation {i}"
-        for sp in gens[-1]:
-            compare_state(e, o, sp, mm.pr)
-        for b in batches:
-            e.free_batch(b)
     with mm.create(engine_lib) as twin:
         for g, specs in enumerate(gens):
             set_calls(g, twin)
@@ -333,8 +307,8 @@ def test_two_slots_in_one_evaluation(engine_lib, oracle_lib, route):
             sp.mats["eigen"][1:] = b.slot
             (le,), (se,) = e.evaluate(sp)
             (lo,), (so,) = o.evaluate(sp)
-            assert se == so == abi.EVAL_OK and rel(le, lo) < tol_of(S), step
-            compare_state(e, o, sp, pr)
+            assert se == so == abi.EVAL_OK and rel(le, lo) < lnl_tol(S), step
+            compare_written(e, o, sp, tree_tol(pr))
             node_of = {int(v): i for i, v in enumerate(pr.chains[0].ti)}
             for j, mu in enumerate(sp.mats):
                 m = a if j == 0 else b
@@ -364,7 +338,7 @@ def test_guard_flag_in_one_evaluation_of_a_batch(engine_lib, oracle_lib, route, 
     with threshold_instance(pr, engine_lib, route, values, kind, c) as e, \
          threshold_instance(pr, oracle_lib, route, values, kind, c) as o:
         o.set_arith(1)
-        (res,) = run_threshold(engine_lib, e, o, route, [specs])
+        (res,) = run_threshold(e, o, route, [specs])
         for i, (le, se, lo, so) in enumerate(res):
             want = abi.EVAL_UNDERFLOW if i == 1 else abi.EVAL_OK
             assert se == so == want, f"evaluation {i}"

@@ -9,28 +9,10 @@ import numpy as np
 import pytest
 from scipy.linalg import expm
 
+from engine_checks import eigen_instance, reversible_q
 from mrbayes_b200 import abi
 
 pytestmark = pytest.mark.gpu
-
-
-def reversible_q(rng, S, sparse=False, skew=False, equal=False):
-    R = rng.gamma(1.0, 1.0, (S, S)) + 0.05
-    if equal:
-        R[:] = 1.0
-    if sparse:                                   # codon-like: most exchanges impossible, chain graph keeps it connected
-        keep = rng.random((S, S)) < 0.15
-        for i in range(S - 1):
-            keep[i, i + 1] = True
-        R = np.where(keep, R, 0.0)
-    R = np.triu(R, 1); R = R + R.T
-    pi = rng.dirichlet(np.full(S, 0.3 if skew else 5.0))
-    pi = np.maximum(pi, 1e-7); pi /= pi.sum()
-    Q = R * pi[None, :]
-    np.fill_diagonal(Q, 0.0)
-    np.fill_diagonal(Q, -Q.sum(1))
-    Q /= -(pi * np.diag(Q)).sum()                # one expected substitution per unit time
-    return Q, pi
 
 
 def cijk_block(Q, pi):
@@ -45,12 +27,6 @@ def cijk_block(Q, pi):
     S = Q.shape[0]
     c = np.einsum("ik,kj->ijk", V, Vi)
     return np.concatenate([lam, np.zeros(S), c.ravel()])
-
-
-def make(lib, S, K, parts):
-    flags = (parts << 8) if parts > 1 else 0
-    return abi.Instance(lib, tip_count=2, partials_count=4, state_count=S, pattern_count=16, category_count=K,
-                        matrix_count=6, scaler_count=2, eigen_count=3, flags=flags)
 
 
 CASES = [
@@ -73,7 +49,7 @@ def test_device_eigensystem_gives_the_matrix_exponential(engine_lib, S, K, parts
     rates = np.ones(K) if parts > 1 else np.linspace(0.2, 2.5, K)
     lengths = [0.004, 0.11, 0.9, 3.7]
     mats = np.zeros(len(lengths), abi.MAT_DTYPE)
-    with make(engine_lib, S, K, parts) as dev, make(engine_lib, S, K, parts) as host:
+    with eigen_instance(engine_lib, S, K, parts) as dev, eigen_instance(engine_lib, S, K, parts) as host:
         dev.set_rate_matrices(1, Qs, pi)
         host.set_cijk(1, np.concatenate([cijk_block(q, pi) for q in Qs]))
         for i, t in enumerate(lengths):
@@ -94,7 +70,7 @@ def test_slots_can_be_rewritten_back_to_back(engine_lib):
     """The staging area of a slot is reused only after its previous copy has been consumed: the LAST matrices win."""
     rng = np.random.default_rng(7)
     S = 61
-    with make(engine_lib, S, 1, 1) as dev:
+    with eigen_instance(engine_lib, S, 1, 1) as dev:
         last = None
         for rep in range(6):
             Q, pi = reversible_q(rng, S, sparse=True)
@@ -113,7 +89,7 @@ def test_slots_can_be_rewritten_back_to_back(engine_lib):
 def test_rejects_what_it_cannot_diagonalise(engine_lib):
     Q, pi = reversible_q(np.random.default_rng(3), 4)
     bad = pi.copy(); bad[2] = 0.0
-    with make(engine_lib, 4, 1, 1) as dev:
+    with eigen_instance(engine_lib, 4, 1, 1) as dev:
         rc = engine_lib.fn("set_rate_matrices")(dev.handle, 0, -1, abi._ptr(np.ascontiguousarray(Q), abi.C.c_double), abi._ptr(bad, abi.C.c_double))
         assert rc != 0
         rc = engine_lib.fn("set_rate_matrices")(dev.handle, 9, -1, abi._ptr(np.ascontiguousarray(Q), abi.C.c_double), abi._ptr(pi, abi.C.c_double))
@@ -134,7 +110,7 @@ def test_warm_started_chain_of_proposals(engine_lib, S, parts):
     R = Q / pi[None, :]; np.fill_diagonal(R, 0.0)          # exchangeabilities
     mats = np.zeros(1, abi.MAT_DTYPE)
     cur = 0
-    with make(engine_lib, S, K, parts) as dev:
+    with eigen_instance(engine_lib, S, K, parts) as dev:
         for link in range(80):
             # a multiplier move on a block of exchangeabilities and a Dirichlet-like nudge of the frequencies
             i, j = rng.integers(0, S, 2)

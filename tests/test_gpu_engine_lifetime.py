@@ -1,7 +1,6 @@
 """GPU: the engine's resources across calls that replace or refuse them -- the variable-state tables and matrix
 buffer set a second time, an allocation the device refuses, and a packed batch freed while an evaluation that
 writes its results there is pending.  The instance must keep computing what a fresh instance computes."""
-import ctypes as C
 import sys
 from pathlib import Path
 
@@ -11,8 +10,8 @@ import pytest
 sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import bench  # noqa: E402
 from mrbayes_b200 import abi, workloads  # noqa: E402
+from engine_checks import rel  # noqa: E402
 from std_problems import make_std_division, model_block, random_block  # noqa: E402
-from test_gpu_parity import rel  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -31,12 +30,6 @@ def std_instance(lib, pr, matrix_length):
     return inst
 
 
-def set_matrix(inst, matrix, block):
-    block = np.ascontiguousarray(block, np.float32)
-    inst.lib.check("set_transition_matrix", inst.lib.fn("set_transition_matrix")(
-        inst.handle, matrix, block.ctypes.data_as(C.POINTER(C.c_float))))
-
-
 def supplied_full_evaluation(pr, insts):
     """chain 0's full evaluation with every branch's block supplied by the caller: the model's matrices in the
     first pr.matrix_length floats of each instance's block, 0.5 in the rest"""
@@ -47,7 +40,7 @@ def supplied_full_evaluation(pr, insts):
         for inst, length in insts:
             padded = np.full(length, 0.5, np.float32)
             padded[:len(blk)] = blk
-            set_matrix(inst, int(m), padded)
+            inst.set_transition_matrix(int(m), padded)
     sp.mats = sp.mats[:0].copy()
     return sp
 
@@ -61,7 +54,7 @@ def test_std_tables_set_again_with_longer_matrices(engine_lib, oracle_lib):
     with std_instance(engine_lib, pr, L) as e, std_instance(engine_lib, pr, L2) as fresh, \
          pr.create(oracle_lib) as o:
         for m in range(6):
-            set_matrix(e, m, random_block(pr, rng))
+            e.set_transition_matrix(m, random_block(pr, rng))
         e.set_pattern_states(pr.state_counts, pr.matrix_offsets, pr.freq_offsets, L2, pr.dummy, pr.uncompressed)
         sp = supplied_full_evaluation(pr, [(e, L2), (fresh, L2), (o, L)])
         (le,), (se,) = e.evaluate(sp)
@@ -91,19 +84,6 @@ def test_refused_matrix_buffer_keeps_the_tables(engine_lib):
         assert s1 == abi.EVAL_OK and l1 == l0, f"before {l0!r}, after the refused call {l1!r}"
 
 
-def replay_begin(lib, inst, batch):
-    assert lib.fn("replay_begin")(inst.handle, batch) == 0
-
-
-def replay_end(lib, inst, n):
-    lnl = np.zeros(n, np.float64)
-    st = np.zeros(n, np.int32)
-    assert lib.fn("replay_end")(inst.handle, lnl.ctypes.data_as(C.POINTER(C.c_double)),
-                                st.ctypes.data_as(C.POINTER(C.c_int))) == 0
-    assert not st.any()
-    return lnl
-
-
 @pytest.mark.parametrize("route", ["resident", "launch"])
 def test_free_batch_refused_while_pending(engine_lib, route):
     """replay_begin, then free_batch on that batch: refused with MB200_ERROR_OUT_OF_RANGE; replay_end still gives
@@ -114,11 +94,12 @@ def test_free_batch_refused_while_pending(engine_lib, route):
     try:
         inst, specs = job.insts[0], job.steps[0][0]
         batch = inst.pack(specs)
-        replay_begin(engine_lib, inst, batch)
+        inst.replay_begin(batch)
         with pytest.raises(abi.AbiError) as err:
             inst.free_batch(batch)
         assert err.value.code == ERROR_OUT_OF_RANGE
-        lnl = replay_end(engine_lib, inst, len(specs))
+        lnl, st = inst.replay_end()
+        assert not st.any()
         want, st = inst.evaluate(specs)
         assert not st.any()
         assert np.array_equal(lnl, want)

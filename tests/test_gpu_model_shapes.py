@@ -21,61 +21,18 @@ calls of branch updates over all chains with every third update rejected, and on
 that reads what the rejections restored.  Every evaluation against the oracle (lnL and status; every partials
 buffer and node and site scaler it wrote, at the generic kernel's tolerances), against the same evaluation sent
 alone to a twin instance (bit for bit), and against the float64 reference after the full evaluations, after the
-last updates and after the rejections.  The kernel counters show the route."""
+last updates and after the rejections.  The kernel counters show the route.  engine_checks.SHAPES_TOL says why the
+partials and node scalers get wider bounds here than on the other generic tests."""
 import numpy as np
 import pytest
 from scipy.linalg import expm
 
 from model_shapes import (CODE_OF_STATES, P_EPS, P_TIMES, SHAPES, ShapeModels, cijk_block, codon_model, codon_q,
                           shape_problem, solver_cases)
+from engine_checks import SHAPES_TOL, SYN_RTOL, check_with_oracle, eigen_instance, num_sms, rel
 from mrbayes_b200 import abi
-from test_gpu_eigen import make
-from test_gpu_parity import SYN_RTOL, rel
-from test_gpu_paths import num_sms
 
 pytestmark = pytest.mark.gpu
-
-# the generic kernel's tolerances of test_gpu_parity._compare_state (S = 20 and 61 run here too, not on the tensor cores),
-# with node scalers at the site scalers' bound and an absolute term for partials (compare_state says why)
-PARTIALS_RTOL, NODE_ATOL, SITE_ATOL = 2e-6, 2e-5, 2e-5
-PARTIALS_OF_PEAK = 2e-7
-
-
-def compare_state(e, o, sp):
-    """Every partials buffer and node scaler sp wrote, and its site scalers, engine against oracle, at the generic
-    kernel's tolerances, except that a partial may also differ by PARTIALS_OF_PEAK times the largest entry of its
-    pattern in the buffer.  That term is the error P(t) brings in: an entry summed from an eigensystem in double is
-    good to ~1e-14 absolute (P_EPS bounds the device eigensolver's), and at these shapes P(t) has entries of 1e-12 and
-    far below (rare codons, short branches, 20 gamma categories).  Where the children of a node disagree, the
-    pattern's largest product is small and the rescaling amplifies such absolute errors.  Measured on an H100 (700 W):
-    partials of 1e-16 to 1e-25 of their pattern's largest differ from the oracle's by up to 7e-3 relative; what exceeds
-    2e-6 relative reaches 5.8e-8 of the pattern's largest with device eigensystems (60 and 63 codons, one Q; 7e-9 at
-    K = 4) and stays below 2e-12 with host eigensystems; entries above 1e-6 of the largest differ by up to 2e-4
-    relative (63 codons, device).  lnL agrees to 1e-8 throughout.  The existing generic tests' dense models with
-    Dirichlet(5) frequencies have no such entries.
-    Node scalers get the site scalers' 2e-5 instead of 1e-6: a child's partials carry that error of up to
-    PARTIALS_OF_PEAK of their largest entry, and a parent whose largest product rests on such entries of the child
-    moves its scaler by their relative error (measured: 7.2e-6 at one pattern of a 60-codon node, device eigensystems,
-    the node's partials and lnL within their bounds).
-    -> (largest relative difference over the entries above 1e-6 of their pattern's largest, largest excess over
-    2e-6 relative as a fraction of the pattern's largest)"""
-    rel_big = rel_max = 0.0
-    for op in sp.ops:
-        a, b = (np.asarray(x, np.float64) for x in (e.get_partials(int(op["dest"])), o.get_partials(int(op["dest"]))))
-        peak = np.abs(b).max(axis=(0, 2), keepdims=True)
-        d = np.abs(a - b)
-        bound = PARTIALS_RTOL * np.abs(b) + PARTIALS_OF_PEAK * peak
-        assert (d <= bound).all(), f"partials of buffer {op['dest']}: {(d / bound).max():.2f} x the bound"
-        big = np.abs(b) > 1e-6 * peak
-        rel_big = max(rel_big, float((d[big] / np.abs(b[big])).max(initial=0.0)))
-        rel_max = max(rel_max, float(((d - PARTIALS_RTOL * np.abs(b)) / np.where(peak > 0, peak, 1.0)).max()))
-        if op["scale_write"] >= 0:
-            d = np.abs(e.get_scalers(int(op["scale_write"])) - o.get_scalers(int(op["scale_write"]))).max()
-            assert d < NODE_ATOL, f"node scaler {op['scale_write']}: {d:.2e}"
-    if sp.site_dst >= 0:
-        d = np.abs(e.get_scalers(sp.site_dst) - o.get_scalers(sp.site_dst)).max()
-        assert d < SITE_ATOL, f"site scaler {sp.site_dst}: {d:.2e}"
-    return rel_big, rel_max
 
 
 # (shape, pattern count: "tp32" = 32 x SMs + 1, else C)
@@ -113,13 +70,9 @@ def test_generic_route_at_production_shape(engine_lib, oracle_lib, name, C):
             for i, sp in enumerate(specs):
                 (la,), (sa,) = twin.evaluate(sp)
                 assert sa == st[i] and la == lnl[i], f"evaluation {i}: alone {la!r}, batched {lnl[i]!r}"
-                (lo,), (so,) = o.evaluate(sp)
-                assert st[i] == so == abi.EVAL_OK, f"evaluation {i} (chain {sp.chain})"
-                r = rel(lnl[i], lo)
-                worst["oracle"] = max(worst["oracle"], r)
-                assert r < SYN_RTOL, f"evaluation {i} (chain {sp.chain}): {r:.2e}"
-                rb, rm = compare_state(e, o, sp)
-                worst["partials"], worst["partials_of_peak"] = max(worst["partials"], rb), max(worst["partials_of_peak"], rm)
+            for k, x in zip(("oracle", "partials", "partials_of_peak"),
+                            check_with_oracle(e, o, specs, lnl, st, SYN_RTOL, SHAPES_TOL)):
+                worst[k] = max(worst[k], x)
             return lnl
 
         against_f64(call([mm.full(ch) for ch in range(n)]))
@@ -169,7 +122,7 @@ def test_device_eigensystem_entry_by_entry(engine_lib, name):
     for i, t in enumerate(P_TIMES):
         mats[i] = (i, 1, t)
     worst = 0.0
-    with make(engine_lib, S, K, parts) as dev, make(engine_lib, S, K, parts) as host:
+    with eigen_instance(engine_lib, S, K, parts) as dev, eigen_instance(engine_lib, S, K, parts) as host:
         dev.set_rate_matrices(1, Qs, pi)
         host.set_cijk(1, cijk_block(Qs, pi))
         dev.update_transition_matrices(mats, rates, pi)
@@ -200,7 +153,7 @@ def test_warm_started_codon_chain(engine_lib):
     _, pi = codon_model(code, rng, kappa, omegas, 1.0)
     mats = np.zeros(1, abi.MAT_DTYPE)
     cur, worst = 0, 0.0
-    with make(engine_lib, S, 3, 3) as dev:
+    with eigen_instance(engine_lib, S, 3, 3) as dev:
         for link in range(40):
             kappa *= np.exp(0.2 * (rng.random() - 0.5))
             omegas = omegas * np.exp(0.2 * (rng.random(3) - 0.5))

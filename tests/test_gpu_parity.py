@@ -1,35 +1,17 @@
 """GPU: the CUDA engine through the C-ABI against (1) the reference's recorded lnL, (2) the
 CPU oracle on identical inputs, (3) size-independent properties at BASELINE.json's full sizes.
 
-Tolerances: lnL 1e-6 relative is the north-star bar (BASELINE.json); what we actually require
-is 100x tighter -- 1e-8 -- because the engine reproduces the reference's float operation order;
-what is left (observed ~1e-9) is the last-bit difference between glibc's and CUDA's log/exp in
-the node scalers and in P(t), the same size as the reference's own SSE-vs-FMA spread.  Conditional likelihoods: 2e-6 relative (a few float ulps: FMA contraction
-and summation order are the only differences allowed), scalers 1e-6 absolute."""
+Tolerances (tests/engine_checks.py): lnL 1e-8 relative, 100x tighter than the north-star bar, on the
+recorded cases; conditional likelihoods 2e-6 relative, node scalers 1e-6 absolute (parity_tol)."""
 import numpy as np
 import pytest
 
 from conftest import GOLDEN, GOLDEN_FILES
+from engine_checks import LNL_RTOL, SYN_RTOL, check_with_oracle, compare_written, evaluation_sequence, lnl_tol, \
+    parity_tol, rel
 from mrbayes_b200 import abi, records, workloads
 
 pytestmark = pytest.mark.gpu
-
-LNL_RTOL = 1e-8
-# synthetic cases have |lnL| of a few hundred and, for S != 4, fused-vs-separate multiply-add
-# differences against the oracle's *_Gen_SSE arithmetic: still 5x inside the north-star bar
-SYN_RTOL = 2e-7
-# 20- and 61-state divisions run on the tensor cores with 3xTF32 operand splitting: each matvec
-# carries ~7e-7 relative error, mostly the tensor core's truncating FP32 accumulation (a small
-# negative bias), which shows up as ~1e-7 relative in lnL -- 5x inside the north-star bar of 1e-6
-TC_RTOL = 5e-7
-
-
-def lnl_tol(S, base):
-    return TC_RTOL if S in (20, 61) else base
-
-
-def rel(a, b):
-    return abs(a - b) / max(abs(b), 1e-300)
 
 
 @pytest.mark.parametrize("stem,arith", GOLDEN_FILES)
@@ -61,17 +43,6 @@ def test_transition_matrices_match_oracle(engine_lib, oracle_lib):
                 n += 1
                 if n >= 3:
                     break
-
-
-def _compare_state(e, o, spec, S):
-    for op in spec.ops:
-        a, b = e.get_partials(int(op["dest"])), o.get_partials(int(op["dest"]))
-        assert np.allclose(a, b, rtol=(2e-5 if S in (20, 61) else 2e-6), atol=1e-37), f"partials of buffer {op['dest']}"
-        if op["scale_write"] >= 0:
-            sa, sb = e.get_scalers(int(op["scale_write"])), o.get_scalers(int(op["scale_write"]))
-            assert np.allclose(sa, sb, atol=1e-6)
-    if spec.site_dst >= 0:
-        assert np.allclose(e.get_scalers(spec.site_dst), o.get_scalers(spec.site_dst), atol=2e-5)
 
 
 CASES = [
@@ -109,26 +80,10 @@ def test_engine_matches_oracle_synthetic(engine_lib, oracle_lib, S, K, C, tips, 
     the same calls; every written buffer compared."""
     nch = 2
     pr = workloads.make_problem(S, K, C, tips, nch, seed=100 + S + K + C, p_invar=pinv, p_ambig=pamb)
-    rng = np.random.default_rng(7)
     with pr.create(engine_lib) as e, pr.create(oracle_lib) as o:
         o.set_arith(1)
-        for ch in range(nch):
-            sp = pr.full_evaluation(ch)
-            (le,), (se,) = e.evaluate(sp)
-            (lo,), (so,) = o.evaluate(sp)
-            assert se == so == abi.EVAL_OK
-            assert rel(le, lo) < lnl_tol(S, SYN_RTOL)
-            _compare_state(e, o, sp, S)
-        for it in range(10):
-            ch = it % nch
-            old = pr.tree[ch].length.copy()
-            sp = pr.random_branch_update(ch, rng)
-            (le,), _ = e.evaluate(sp)
-            (lo,), _ = o.evaluate(sp)
-            assert rel(le, lo) < lnl_tol(S, SYN_RTOL), f"iteration {it}"
-            _compare_state(e, o, sp, S)
-            if it % 3 == 2:
-                pr.reject(ch, sp, old)
+        for _, sp in evaluation_sequence(pr, 10, seed=7):
+            check_with_oracle(e, o, [sp], *e.evaluate(sp), lnl_tol(S), parity_tol(S))
 
 
 @pytest.mark.parametrize("S,K,C,tips", [(4, 4, 413, 12), (20, 4, 64, 6), (61, 1, 40, 5)])
@@ -263,7 +218,7 @@ def test_time_min_and_time_max_branches_other_state_counts(engine_lib, oracle_li
         o.set_arith(1)
         sp = pr.full_evaluation(0)
         (le,), _ = e.evaluate(sp); (lo,), _ = o.evaluate(sp)
-        assert rel(le, lo) < lnl_tol(S, SYN_RTOL)
+        assert rel(le, lo) < lnl_tol(S)
         P0 = e.get_transition_matrix(int(pr.chains[0].ti[0]))
         assert np.array_equal(P0, np.broadcast_to(np.eye(S, dtype=np.float32), P0.shape))
         P1 = e.get_transition_matrix(int(pr.chains[0].ti[1]))
@@ -338,7 +293,7 @@ def test_large_trees_span_several_chunks(engine_lib, oracle_lib, tips, K):
         sp = pr.full_evaluation(0)
         (le,), _ = e.evaluate(sp); (lo,), _ = o.evaluate(sp)
         assert rel(le, lo) < SYN_RTOL
-        _compare_state(e, o, sp, 4)
+        compare_written(e, o, sp, parity_tol(4))
         for it in range(6):
             sp = pr.random_branch_update(0, rng)
             (le,), _ = e.evaluate(sp); (lo,), _ = o.evaluate(sp)
@@ -424,25 +379,12 @@ def test_variable_state_engine_matches_oracle(engine_lib, oracle_lib, C, K, tips
     pr = workloads.make_std_problem(C, K, tips, nch, seed=900 + C + K + smax, max_states=smax, dummy=dummy)
     rng = np.random.default_rng(11)
     with pr.create(engine_lib) as e, pr.create(oracle_lib) as o:
-        for ch in range(nch):
-            sp = pr.full_evaluation(ch)
-            (le,), (se,) = e.evaluate(sp)
-            (lo,), (so,) = o.evaluate(sp)
-            assert se == so == abi.EVAL_OK
-            assert rel(le, lo) < 1e-9
-            for m in sp.mats["matrix"][:5]:
-                assert np.allclose(e.get_transition_matrix(int(m)), o.get_transition_matrix(int(m)), rtol=2.5e-7, atol=1e-30)
-            _compare_state(e, o, sp, smax)
-        for it in range(12):
-            ch = it % nch
-            old = pr.tree[ch].length.copy()
-            sp = pr.random_branch_update(ch, rng)
-            (le,), _ = e.evaluate(sp)
-            (lo,), _ = o.evaluate(sp)
-            assert rel(le, lo) < 1e-9, f"iteration {it}"
-            _compare_state(e, o, sp, smax)
-            if it % 3 == 2:
-                pr.reject(ch, sp, old)
+        for it, sp in evaluation_sequence(pr, 12, seed=rng):
+            check_with_oracle(e, o, [sp], *e.evaluate(sp), 1e-9, parity_tol(smax))
+            if it < 0:
+                for m in sp.mats["matrix"][:5]:
+                    assert np.allclose(e.get_transition_matrix(int(m)), o.get_transition_matrix(int(m)), rtol=2.5e-7,
+                                       atol=1e-30)
         assert e.kernel_launches(abi.KERNEL_STD) == nch + 12        # the variable-state kernel served every call
         # all chains of a generation in one launch == one call per chain
         sps = [pr.random_branch_update(ch, rng) for ch in range(nch)]
@@ -463,8 +405,7 @@ def test_variable_state_general_matrices(engine_lib, oracle_lib):
         assert rel(l0, o0) < 1e-9
         # re-load one matrix unchanged: same lnL through the general path
         m = int(sp.mats["matrix"][0])
-        e.lib.check("set_transition_matrix", e.lib.fn("set_transition_matrix")(
-            e.handle, m, e.get_transition_matrix(m).ctypes.data_as(abi.C.POINTER(abi.C.c_float))))
+        e.set_transition_matrix(m, e.get_transition_matrix(m))
         sp2 = abi.EvalSpec(ops=sp.ops[-1:].copy(), site_dst=sp.site_dst, site_src=sp.site_dst, root=sp.root, rates=sp.rates,
                            cat_weights=sp.cat_weights, freqs=sp.freqs)
         sp2.ops["scale_remove"] = abi.NONE

@@ -19,126 +19,27 @@ The threshold between the fused and the non-fused 4-state path scales with the d
 so the pattern counts here are computed from it."""
 import numpy as np
 import pytest
-import torch
 
-from f64_reference import caterpillar_tree, f64_lnl, tree_height
+from engine_checks import (DBL_MAX, SYN_RTOL, TC_RTOL, assert_resident_equals_launches, check_with_oracle,
+                           dead_pattern_problem, edge, evaluation_sequence, kernel_names, launched, lnl_tol, num_sms,
+                           nuc4_problem, parity_tol, ppb, rel, resident_generations, tree_tol, via_evaluate, via_replay)
+from f64_reference import caterpillar_tree, f64_lnl
 from mrbayes_b200 import abi, workloads
-from test_gpu_parity import SYN_RTOL, TC_RTOL, _compare_state, rel
 
 pytestmark = pytest.mark.gpu
 
-DBL_MAX = np.finfo(np.float64).max
 
-
-def num_sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def ppb(K):
-    """patterns per 4-state tile: 256 threads / pow2ceil(K) lanes per pattern"""
-    return 256 // (1 << (K - 1).bit_length())
-
-
-def edge(K, tiles):
-    """a pattern count at a tile edge: exactly `tiles` tiles, or one pattern less or more (rotating with K)"""
-    return tiles * ppb(K) + (K % 3) - 1
-
-
-def kernel_names(fn, expect):
-    """names of the CUDA kernels fn() launches (CUDA activity trace, no hardware counters), for what the
-    kernel counters cannot tell: the K and parameter-block size of a 4-state instantiation.  The trace
-    can miss launches, so fn -- a full evaluation, which is idempotent -- is traced up to three times
-    until a kernel whose name contains `expect` shows up."""
-    from torch.profiler import ProfilerActivity, profile
-    for _ in range(3):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            fn()
-            torch.cuda.synchronize()
-        names = {e.name for e in prof.events() if str(e.device_type).endswith("CUDA")}
-        if launched(names, expect):
-            break
-    return names
-
-
-def launched(names, prefix):
-    return any(prefix in n for n in names)
-
-
-# ---- routes: how a list of evaluations reaches the engine ---------------------------------
-def via_evaluate(e, specs):
-    return e.evaluate(specs)
-
-
-def via_replay(e, specs):
-    b = e.pack(specs)
-    e.replay(b)
-    out = e.replay_results(b, len(specs))
-    e.free_batch(b)
-    return out
-
-
-def compare_state(e, o, spec, pr):
-    """_compare_state of the parity suite.  On the tensor-core path the 3xTF32 rounding of each level
-    (up to ~1e-6 relative) adds up from the tips to the node: on H100, S = 61 and K = 3, the partials
-    of a node 20 to 38 levels up differ from the oracle's by 2e-5, the parity suite's bound for its
-    trees of a few levels.  So the partials and the node scalers (the log of the node's largest
-    unscaled partial) get 2e-5 plus 1e-6 per level of the tree."""
-    if pr.S not in (20, 61):
-        return _compare_state(e, o, spec, pr.S)
-    tol = 2e-5 + 1e-6 * tree_height(pr.tree[spec.chain])
-    for op in spec.ops:
-        a, b = e.get_partials(int(op["dest"])), o.get_partials(int(op["dest"]))
-        assert np.allclose(a, b, rtol=tol, atol=1e-37), f"partials of buffer {op['dest']}"
-        if op["scale_write"] >= 0:
-            d = np.abs(e.get_scalers(int(op["scale_write"])) - o.get_scalers(int(op["scale_write"]))).max()
-            assert d < tol, f"node scaler {op['scale_write']}: {d:.2e}"
-    if spec.site_dst >= 0:
-        assert np.allclose(e.get_scalers(spec.site_dst), o.get_scalers(spec.site_dst), atol=2e-5 + tol)
-
-
-def tol_of(S):
-    return TC_RTOL if S in (20, 61) else SYN_RTOL
-
-
-def check_run(pr, e, o, route, updates, seed, chains=(0, 1)):
+def check_run(pr, e, o, route, updates, seed):
     """A full evaluation per chain, then `updates` branch updates over the chains with a rejection
     every third: lnL, every written partials buffer and the node and site scalers against the oracle;
     lnL against the float64 reference after the full evaluations and after the last update."""
-    tol = tol_of(pr.S)
-    for ch in chains:
-        sp = pr.full_evaluation(ch)
-        (le,), (se,) = route(e, [sp])
-        (lo,), (so,) = o.evaluate(sp)
-        assert se == so == abi.EVAL_OK
-        assert rel(le, lo) < tol, f"full evaluation of chain {ch}"
-        compare_state(e, o, sp, pr)
-        r = rel(le, f64_lnl(pr, ch)[1])
-        assert r < tol, f"float64 reference, chain {ch}: {r:.2e}"
-    rng = np.random.default_rng(seed)
-    for it in range(updates):
-        ch = chains[it % len(chains)]
-        old = pr.tree[ch].length.copy()
-        sp = pr.random_branch_update(ch, rng)
-        (le,), (se,) = route(e, [sp])
-        (lo,), _ = o.evaluate(sp)
-        assert se == abi.EVAL_OK and rel(le, lo) < tol, f"update {it}"
-        compare_state(e, o, sp, pr)
-        if it == updates - 1:
-            r = rel(le, f64_lnl(pr, ch)[1])
-            assert r < tol, f"float64 reference after the updates: {r:.2e}"
-        elif it % 3 == 2:
-            pr.reject(ch, sp, old)
-
-
-def nuc4_problem(K, C, n_chains=2, seed=0, tips=40):
-    """4-state problem whose chain 1 is a caterpillar (one node per level: many chunks); odd K carry
-    p_invar and partial ambiguity"""
-    odd = K % 2 == 1
-    pr = workloads.make_problem(4, K, C, tips, n_chains, seed=1000 + 17 * K + seed,
-                                p_invar=0.15 if odd else 0.0, p_ambig=0.1 if odd else 0.0)
-    pr.tree[1] = caterpillar_tree(tips, np.random.default_rng(K))
-    return pr
+    tol = lnl_tol(pr.S)
+    for it, sp in evaluation_sequence(pr, updates, seed):
+        lnl, st = route(e, [sp])
+        check_with_oracle(e, o, [sp], lnl, st, tol, tree_tol(pr))
+        if it < 0 or it == updates - 1:
+            r = rel(lnl[0], f64_lnl(pr, sp.chain)[1])
+            assert r < tol, f"float64 reference after evaluation {it} (chain {sp.chain}): {r:.2e}"
 
 
 # ---- B. 4-state path matrix -------------------------------------------------------------
@@ -170,11 +71,7 @@ def test_nuc4_parameter_block_sizes(engine_lib, oracle_lib, cap, K, tips, n_eval
                 names = kernel_names(lambda: e.evaluate(specs), want)
                 assert launched(names, want), names
             lnl, st = e.evaluate(specs)
-            assert not st.any()
-            for i, sp in enumerate(specs):
-                (lo,), _ = o.evaluate(sp)
-                assert rel(lnl[i], lo) < SYN_RTOL
-                _compare_state(e, o, sp, 4)
+            check_with_oracle(e, o, specs, lnl, st, SYN_RTOL, parity_tol(4))
         assert rel(lnl[-1], f64_lnl(pr, n_eval - 1)[1]) < SYN_RTOL
 
 
@@ -219,48 +116,7 @@ def test_nuc4_resident_equals_launches(engine_lib, oracle_lib, K):
         if g % 3 == 2:
             for ch in (0, 1):
                 pr.reject(ch, gens[-1][ch], old[ch])
-    dests = sorted({int(op["dest"]) for s in gens for sp in s for op in sp.ops})
-    scal = sorted({int(op["scale_write"]) for s in gens for sp in s for op in sp.ops if op["scale_write"] >= 0} |
-                  {int(sp.site_dst) for s in gens for sp in s})
-
-    def final_state(e):
-        return [e.get_partials(b) for b in dests], [e.get_scalers(s) for s in scal]
-
-    want = []
-    with pr.create(engine_lib) as e, pr.create(oracle_lib) as o:
-        o.set_arith(1)
-        for specs in gens:
-            b = e.pack(specs)
-            e.replay(b)
-            lnl, st = e.replay_results(b, 2)
-            e.free_batch(b)
-            assert not st.any()
-            for i, sp in enumerate(specs):
-                (lo,), _ = o.evaluate(sp)
-                assert rel(lnl[i], lo) < SYN_RTOL
-                _compare_state(e, o, sp, 4)
-            want.append(lnl)
-        assert rel(want[-1][1], f64_lnl(pr, 1)[1]) < SYN_RTOL
-        want_state = final_state(e)
-    with pr.create(engine_lib) as e:
-        batches = [e.pack(specs) for specs in gens]
-        n0 = e.launch_count()
-        got = []
-        for b in batches:
-            assert engine_lib.fn("replay_begin")(e.handle, b) == 0
-            lnl = np.zeros(2, np.float64)
-            st = np.zeros(2, np.int32)
-            assert engine_lib.fn("replay_end")(e.handle, lnl.ctypes.data_as(abi.C.POINTER(abi.C.c_double)),
-                                              st.ctypes.data_as(abi.C.POINTER(abi.C.c_int))) == 0
-            assert not st.any()
-            got.append(lnl)
-        launches = e.launch_count() - n0
-        e.synchronize()
-        got_state = final_state(e)
-    assert launches < len(gens)                      # one kernel served several generations
-    assert np.array_equal(np.array(got), np.array(want))
-    assert all(np.array_equal(a, b) for a, b in zip(got_state[0], want_state[0]))
-    assert all(np.array_equal(a, b) for a, b in zip(got_state[1], want_state[1]))
+    assert_resident_equals_launches(engine_lib, oracle_lib, pr, gens, SYN_RTOL, parity_tol(4))
 
 
 @pytest.mark.parametrize("K", range(1, 9))
@@ -274,11 +130,7 @@ def test_nuc4_throughput_mode(engine_lib, oracle_lib, K):
         for gen in range(4):
             specs = [pr.full_evaluation(ch) if gen == 0 else pr.random_branch_update(ch, rng) for ch in range(nch)]
             lnl, st = e.evaluate(specs)
-            assert not st.any()
-            for i, sp in enumerate(specs):
-                (lo,), _ = o.evaluate(sp)
-                assert rel(lnl[i], lo) < SYN_RTOL
-                _compare_state(e, o, sp, 4)
+            check_with_oracle(e, o, specs, lnl, st, SYN_RTOL, parity_tol(4))
         assert rel(lnl[0], f64_lnl(pr, 0)[1]) < SYN_RTOL
 
 
@@ -303,32 +155,23 @@ def test_tensor_core_matrix(engine_lib, oracle_lib, S, K, C):
         # all chains' full evaluations in one call
         specs = [pr.full_evaluation(ch) for ch in range(nch)]
         lnl, st = e.evaluate(specs)
-        assert not st.any()
-        for ch, sp in enumerate(specs):
-            (lo,), _ = o.evaluate(sp)
-            assert rel(lnl[ch], lo) < TC_RTOL, f"chain {ch}"
-            if ch < 2:
-                compare_state(e, o, sp, pr)
-                r = rel(lnl[ch], f64_lnl(pr, ch)[1])
-                assert r < TC_RTOL, f"float64 reference, chain {ch}: {r:.2e}"
+        check_with_oracle(e, o, specs, lnl, st, TC_RTOL, tree_tol(pr))
+        for ch in range(2):
+            r = rel(lnl[ch], f64_lnl(pr, ch)[1])
+            assert r < TC_RTOL, f"float64 reference, chain {ch}: {r:.2e}"
         for it in range(10):
             ch = it % 2
             old = pr.tree[ch].length.copy()
             sp = pr.random_branch_update(ch, rng)
-            (le,), (se,) = e.evaluate(sp)
-            (lo,), _ = o.evaluate(sp)
-            assert se == abi.EVAL_OK and rel(le, lo) < TC_RTOL, f"update {it}"
-            compare_state(e, o, sp, pr)
+            check_with_oracle(e, o, [sp], *e.evaluate(sp), TC_RTOL, tree_tol(pr))
             if it % 3 == 2:
                 pr.reject(ch, sp, old)
         # one generation of branch updates over all chains in one call
         specs = [pr.random_branch_update(ch, rng) for ch in range(nch)]
         assert len({len(sp.ops) for sp in specs}) > 1
         lnl, st = e.evaluate(specs)
-        assert not st.any()
-        for ch, sp in enumerate(specs):
-            (lo,), _ = o.evaluate(sp)
-            assert rel(lnl[ch], lo) < TC_RTOL, f"batched update, chain {ch}"
+        check_with_oracle(e, o, specs, lnl, st, TC_RTOL, tree_tol(pr))
+        for ch in range(nch):
             r = rel(lnl[ch], f64_lnl(pr, ch)[1])
             assert r < TC_RTOL, f"float64 reference, batched update, chain {ch}: {r:.2e}"
         assert e.kernel_launches(abi.KERNEL_TENSOR) == 12
@@ -403,34 +246,6 @@ def test_time_limits_std(engine_lib, oracle_lib):
 
 
 # ---- F. underflow across tiles and evaluations -----------------------------------------------
-def dead_pattern_problem(family, where, n_chains=1):
-    """Every pattern compatible (all tips in one state) except pattern `dead`, where the root tip
-    disagrees; with P = I (branches below TIME_MIN) that pattern's likelihood is exactly 0."""
-    sms = num_sms()
-    if family == "std":
-        C = 64 * 5 + 1 if where == "last" else 64 * 5       # K = 2: 64 patterns per tile
-        pr = workloads.make_std_problem(C, 2, 6, n_chains, seed=7, max_states=5, dummy=0)
-        pr.rates = pr.rates * 1e-10          # Std clamps lengths up to BRLENS_MIN: P = I needs r t < 1e-17
-        pr.masks[:] = 1
-        base = np.zeros(C, np.int64)
-    else:
-        S, K, C, tile = {"nuc4_host": (4, 4, 10 * 64, 64), "nuc4_device": (4, 4, 40 * 64, 64),
-                         "nuc4_non_fused": (4, 4, (4 * sms + 4) * 64, 64), "nuc4_resident": (4, 4, 12 * 64, 64),
-                         "nuc4_throughput": (4, 4, 10 * 64, 64), "tensor": (20, 2, 4 * 128, 128),
-                         "generic": (16, 2, 300, 4)}[family]
-        if where == "last":
-            C -= tile - 1                      # the last tile holds one pattern
-        pr = workloads.make_problem(S, K, C, 6, n_chains, seed=8, p_missing=0.0)
-        base = np.random.default_rng(1).integers(0, S, size=C)
-        pr.masks[:] = (np.uint64(1) << base.astype(np.uint64))[None, :]
-    # the root tip disagrees with the rest: every interior node below the root keeps a non-zero
-    # (scalable) likelihood, the zero appears where the interior root combines its three children
-    dead = C - 1 if where == "last" else C // 2 + 1
-    pr.masks[:, dead] = np.uint64(1) << np.uint64(base[dead])
-    pr.masks[pr.tree[0].root, dead] = np.uint64(1) << np.uint64((base[dead] + 1) % 2)
-    return pr, dead
-
-
 FAMILIES = ["nuc4_host", "nuc4_device", "nuc4_non_fused", "nuc4_resident", "nuc4_throughput", "tensor", "generic", "std"]
 KIND = {"nuc4_host": abi.KERNEL_NUC4, "nuc4_device": abi.KERNEL_NUC4, "nuc4_non_fused": abi.KERNEL_NUC4,
         "nuc4_resident": abi.KERNEL_NUC4, "nuc4_throughput": abi.KERNEL_NUC4,
@@ -441,28 +256,11 @@ def family_instance(pr, lib, family):
     return pr.create(lib, flags=abi.CONFIG_THROUGHPUT if family == "nuc4_throughput" else 0)
 
 
-def resident_generations(lib, e, gens):
-    """generations through replay_begin / _end, all packed first (packing retires a resident kernel)
-    -> [(lnL, status)] per generation"""
-    batches = [e.pack(specs) for specs in gens]
-    out = []
-    for b, specs in zip(batches, gens):
-        lnl = np.zeros(len(specs), np.float64)
-        st = np.zeros(len(specs), np.int32)
-        assert lib.fn("replay_begin")(e.handle, b) == 0
-        assert lib.fn("replay_end")(e.handle, lnl.ctypes.data_as(abi.C.POINTER(abi.C.c_double)),
-                                    st.ctypes.data_as(abi.C.POINTER(abi.C.c_int))) == 0
-        out.append((lnl, st))
-    for b in batches:
-        e.free_batch(b)
-    return out
-
-
-def family_evaluate(lib, e, family, specs):
+def family_evaluate(e, family, specs):
     """e.evaluate, or for nuc4_resident one generation through replay_begin / _end"""
     if family != "nuc4_resident":
         return e.evaluate(specs)
-    return resident_generations(lib, e, [specs])[0]
+    return resident_generations(e, [specs])[0]
 
 
 @pytest.mark.parametrize("where", ["middle", "last"])
@@ -478,7 +276,7 @@ def test_underflow_in_one_tile(engine_lib, oracle_lib, family, where):
         sp = pr.full_evaluation(0)
         if family == "nuc4_resident":
             alive = pr.branch_update(0, pr.tree[0].root_left, 0.1)
-            ((le,), (se,)), ((la,), (sa,)) = resident_generations(engine_lib, e, [[sp], [alive]])
+            ((le,), (se,)), ((la,), (sa,)) = resident_generations(e, [[sp], [alive]])
         else:
             (le,), (se,) = e.evaluate(sp)
         (lo,), (so,) = o.evaluate(sp)
@@ -501,7 +299,7 @@ def test_underflow_in_one_evaluation_of_a_batch(engine_lib, oracle_lib, family):
     with family_instance(pr, engine_lib, family) as e, pr.create(oracle_lib) as o:
         o.set_arith(1)
         specs = [pr.full_evaluation(ch) for ch in range(nch)]
-        lnl, st = family_evaluate(engine_lib, e, family, specs)
+        lnl, st = family_evaluate(e, family, specs)
         assert e.kernel_launches(KIND[family]) == 1
         for ch, sp in enumerate(specs):
             (lo,), (so,) = o.evaluate(sp)
@@ -509,4 +307,4 @@ def test_underflow_in_one_evaluation_of_a_batch(engine_lib, oracle_lib, family):
             if ch == 2:
                 assert lnl[ch] == lo == -DBL_MAX
             else:
-                assert rel(lnl[ch], lo) < tol_of(pr.S), f"chain {ch}"
+                assert rel(lnl[ch], lo) < lnl_tol(pr.S), f"chain {ch}"

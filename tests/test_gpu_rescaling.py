@@ -5,7 +5,8 @@ scaler without writing a new one.  The dynamic rescaling scheme does both (tests
 builds its operation lists), and asks for the guard on 4-state divisions.  Each test here shows the
 route it took (kernel counters) and compares with the CPU oracle (set_arith(1)) and with the float64
 reference.  Partials can be tiny when nodes go unscaled, so they are compared with a relative
-tolerance and an absolute floor of 1e-44 (the subnormal range), not the parity suite's 1e-37.
+tolerance and an absolute floor of 1e-44 (the subnormal range), not the parity suite's 1e-37
+(engine_checks.sparse_tol).
 
   sparse parity      f in {1, 2, 3, 7, inf} on the 4-state routes, tensor core, generic kernel, Std
   deep subtrees      an 80-tip caterpillar with the guard off: scale4's division branch (a maximum
@@ -16,42 +17,17 @@ tolerance and an absolute floor of 1e-44 (the subnormal range), not the parity s
 import numpy as np
 import pytest
 
-from f64_reference import caterpillar_tree, f64_lnl, tree_height
+from engine_checks import (DBL_MAX, SYN_RTOL, assert_resident_equals_launches, check_with_oracle, compare_written,
+                           edge, evaluation_sequence, lnl_tol, num_sms, nuc4_problem, ppb, rel, sparse_tol,
+                           via_evaluate, via_replay)
+from f64_reference import caterpillar_tree, f64_lnl
 from mrbayes_b200 import abi, workloads
-from sparse_rescaling import deep_problem, sparse_rescaling, step_frequency, unscaled_maxima
-from test_gpu_parity import SYN_RTOL, rel
-from test_gpu_paths import edge, num_sms, nuc4_problem, ppb, resident_generations, tol_of, via_evaluate, via_replay
+from sparse_rescaling import (GUARD_MIN, deep_problem, run_threshold, sparse_rescaling, step_frequency,
+                              threshold_instance, threshold_setup, threshold_spec, unscaled_maxima)
 
 pytestmark = pytest.mark.gpu
 
 FREQS = [1, 2, 3, 7, np.inf]
-GUARD_MIN = np.float32(1e-24)
-DBL_MAX = np.finfo(np.float64).max
-FLT_MIN = float(np.finfo(np.float32).tiny)
-
-
-def compare_buffers(e, o, sp, pr):
-    """every buffer sp writes against the oracle: partials relative (tensor core: 2e-5 plus 1e-6
-    per tree level, as test_gpu_paths) with an absolute floor of 1e-44 -- on the tensor core the
-    smallest normal float, because its products flush subnormals: an entry just above 1e-38 loses
-    the terms below (on H100, 5.7e-38 differed by 8e-5 relative); node scalers to 1e-6 plus
-    two float ulps of their size (a sparse scaler is the log of a small maximum: -55 has an ulp of
-    4e-6); site scalers to 2e-5 plus two ulps"""
-    tc = pr.S in (20, 61)
-    ptol = 2e-5 + 1e-6 * tree_height(pr.tree[sp.chain]) if tc else 2e-6
-    stol = ptol if tc else 1e-6
-    floor = FLT_MIN if tc else 1e-44
-    for op in sp.ops:
-        a, b = e.get_partials(int(op["dest"])), o.get_partials(int(op["dest"]))
-        bad = ~np.isclose(a, b, rtol=ptol, atol=floor)
-        assert not bad.any(), (f"partials of buffer {op['dest']}: {bad.sum()} entries, e.g. {a[bad][:3]} vs {b[bad][:3]}; "
-                               f"pattern maxima {b.max(axis=(0, 2))[np.nonzero(bad)[1][:3]]}")
-        if op["scale_write"] >= 0:
-            a, b = e.get_scalers(int(op["scale_write"])), o.get_scalers(int(op["scale_write"]))
-            assert np.allclose(a, b, rtol=2.5e-7, atol=stol), f"node scaler {op['scale_write']}"
-    if sp.site_dst >= 0:
-        a, b = e.get_scalers(sp.site_dst), o.get_scalers(sp.site_dst)
-        assert np.allclose(a, b, rtol=2.5e-7, atol=2e-5 + stol), "site scalers"
 
 
 def remove_only(sp):
@@ -62,29 +38,16 @@ def sparse_run(pr, e, o, route, f, updates=10, seed=0):
     """A full evaluation per chain, then `updates` branch updates (the frequency stepping between f
     and f + 1) with every third rejected: status, lnL and every written buffer against the oracle,
     lnL against float64 (not for Std) after each full evaluation and the last update.  -> calls made"""
-    tol = tol_of(pr.S)
+    tol = lnl_tol(pr.S)
     calls = n_remove_only = 0
-    rng = np.random.default_rng(seed)
-    for it in range(-pr.n_chains, updates):
-        ch = it % pr.n_chains
-        old = pr.tree[ch].length.copy()
-        if it < 0:
-            sp = pr.full_evaluation(ch)
-        else:
-            step_frequency(pr, f, it)
-            sp = pr.random_branch_update(ch, rng)
-        (le,), (se,) = route(e, [sp])
-        (lo,), (so,) = o.evaluate(sp)
+    for it, sp in evaluation_sequence(pr, updates, seed, before_update=lambda it: step_frequency(pr, f, it)):
+        lnl, st = route(e, [sp])
         calls += 1
         n_remove_only += remove_only(sp)
-        assert se == so == abi.EVAL_OK, f"evaluation {it}"
-        assert rel(le, lo) < tol, f"evaluation {it}: {rel(le, lo):.2e}"
-        compare_buffers(e, o, sp, pr)
+        check_with_oracle(e, o, [sp], lnl, st, tol, sparse_tol(pr))
         if (it < 0 or it == updates - 1) and not isinstance(pr, workloads.StdProblem):
-            r = rel(le, f64_lnl(pr, ch)[1])
+            r = rel(lnl[0], f64_lnl(pr, sp.chain)[1])
             assert r < tol, f"float64 reference, evaluation {it}: {r:.2e}"
-        if 0 <= it < updates - 1 and it % 3 == 2:
-            pr.reject(ch, sp, old)
     assert (n_remove_only > 0) == (1 < f < np.inf)           # the lists hold remove-only operations
     return calls
 
@@ -130,45 +93,7 @@ def test_sparse_nuc4_resident_equals_launches(engine_lib, oracle_lib, K, f):
             for ch in (0, 1):
                 pr.reject(ch, gens[-1][ch], old[ch])
     assert (sum(remove_only(sp) for s in gens for sp in s) > 0) == (1 < f < np.inf)
-    dests = sorted({int(op["dest"]) for s in gens for sp in s for op in sp.ops})
-    scal = sorted({int(op["scale_write"]) for s in gens for sp in s for op in sp.ops if op["scale_write"] >= 0} |
-                  {int(sp.site_dst) for s in gens for sp in s})
-
-    def final_state(e):
-        return [e.get_partials(b) for b in dests], [e.get_scalers(s) for s in scal]
-
-    want = []
-    with pr.create(engine_lib) as e, pr.create(oracle_lib) as o:
-        o.set_arith(1)
-        for specs in gens:
-            lnl, st = via_replay(e, specs)
-            assert not st.any()
-            for i, sp in enumerate(specs):
-                (lo,), _ = o.evaluate(sp)
-                assert rel(lnl[i], lo) < SYN_RTOL
-                compare_buffers(e, o, sp, pr)
-            want.append(lnl)
-        assert rel(want[-1][1], f64_lnl(pr, 1)[1]) < SYN_RTOL
-        want_state = final_state(e)
-    with pr.create(engine_lib) as e:
-        batches = [e.pack(specs) for specs in gens]
-        n0 = e.launch_count()
-        got = []
-        for b in batches:
-            lnl = np.zeros(2, np.float64)
-            st = np.zeros(2, np.int32)
-            assert engine_lib.fn("replay_begin")(e.handle, b) == 0
-            assert engine_lib.fn("replay_end")(e.handle, lnl.ctypes.data_as(abi.C.POINTER(abi.C.c_double)),
-                                              st.ctypes.data_as(abi.C.POINTER(abi.C.c_int))) == 0
-            assert not st.any()
-            got.append(lnl)
-        launches = e.launch_count() - n0
-        e.synchronize()
-        got_state = final_state(e)
-    assert launches < len(gens)                      # one kernel served several generations
-    assert np.array_equal(np.array(got), np.array(want))
-    assert all(np.array_equal(a, b) for a, b in zip(got_state[0], want_state[0]))
-    assert all(np.array_equal(a, b) for a, b in zip(got_state[1], want_state[1]))
+    assert_resident_equals_launches(engine_lib, oracle_lib, pr, gens, SYN_RTOL, sparse_tol(pr))
 
 
 @pytest.mark.parametrize("f", FREQS)
@@ -212,7 +137,7 @@ def test_deep_unscaled_subtrees(engine_lib, oracle_lib, route, f):
             (lo,), (so,) = o.evaluate(sp)
             assert se == so, f"evaluation {it}"
             assert rel(le, lo) < SYN_RTOL, f"evaluation {it}: {rel(le, lo):.2e}"
-            compare_buffers(e, o, sp, pr)
+            compare_written(e, o, sp, sparse_tol(pr))
             if f <= 50:
                 r = rel(le, f64_lnl(pr, 0)[1])
                 assert r < SYN_RTOL, f"float64 reference, evaluation {it}: {r:.2e}"
@@ -278,66 +203,6 @@ def test_guard_contract(engine_lib, oracle_lib, record_property, K, tips, f):
 # ---- guard threshold, exact ------------------------------------------------------------------------
 THRESHOLD_VALUES = [(GUARD_MIN, abi.EVAL_OK), (np.nextafter(GUARD_MIN, np.float32(0)), abi.EVAL_UNDERFLOW),
                     (np.float32(1.00003e-24), abi.EVAL_OK)]
-THRESHOLD_C = {"host": 10, "device": 40, "non_fused": None, "throughput": 10, "resident": 12}   # resident: <= 16 tiles
-
-
-def threshold_setup(route, K, where, n_eval):
-    """n_eval evaluations of one node each over 4 tips (buffers and slots of chain e for evaluation e):
-    the node multiplies interior buffers x and 1.0 through P = I (branch length 0).  -> problem, C,
-    the pattern that will carry the value"""
-    tiles = THRESHOLD_C[route] or 4 * num_sms() + 4
-    C = tiles * ppb(K) - (ppb(K) - 1 if where == "last" else 0)
-    pr = workloads.make_problem(4, K, C, 4, n_eval, seed=12, flags=abi.FLAG_NUC4_PINVAR_QUIRK | abi.FLAG_RANGE_GUARD)
-    pr.freqs = np.full(4, 0.25)
-    return pr, C, (C - 1 if where == "last" else C // 2 + 1)
-
-
-def threshold_spec(pr, e_idx, kind):
-    """kind 'node': buffer a -> rescaled node d1 -> unscaled root d2; kind 'root': a -> unscaled root d1"""
-    nI = pr.n_int
-    a, ones, d1, d2 = (pr.n_tips + 2 * e_idx * nI + j for j in range(4))
-    mat = 2 * e_idx * pr.n_nodes
-    base = 2 * e_idx * (nI + 1)
-    op = lambda dest, c1, sw: (dest, c1, mat, ones, mat, abi.NONE, abi.NONE, sw, abi.NONE)
-    ops = [op(d1, a, base), op(d2, d1, abi.NONE)] if kind == "node" else [op(d1, a, abi.NONE)]
-    return abi.EvalSpec(mats=np.array([(mat, 0, 0.0)], abi.MAT_DTYPE), ops=np.array(ops, abi.OP_DTYPE),
-                        site_dst=base + 1, site_src=abi.NONE, root=ops[-1][0], flags=pr.flags,
-                        rates=pr.rates, cat_weights=np.full(pr.K, 1.0 / pr.K), freqs=pr.freqs, chain=e_idx)
-
-
-def threshold_partials(pr, kind, c, x):
-    """'node': 0.5 everywhere but x at pattern c -- its maximum; 'root' (K = 1, frequencies 1/4):
-    1.0 everywhere but x in every state of c, so that likeF = 4 (x / 4) = x exactly"""
-    a = np.full((pr.K, pr.C, 4), 0.5 if kind == "node" else 1.0, np.float32)
-    if x is not None:
-        a[:, c, :] = x
-    return a
-
-
-def run_threshold(engine_lib, e, o, route, gens):
-    """each generation (a list of evaluations) on the route and on the oracle -> [(lnL, status, oracle
-    lnL, oracle status)] per evaluation, per generation.  The resident route packs every generation
-    first, so that one kernel can serve them all."""
-    if route == "resident":
-        got = resident_generations(engine_lib, e, gens)
-    else:
-        got = [(via_replay if route == "device" else via_evaluate)(e, specs) for specs in gens]
-    out = []
-    for (lnl, st), specs in zip(got, gens):
-        out.append([(lnl[i], st[i]) + tuple(x[0] for x in o.evaluate(sp)) for i, sp in enumerate(specs)])
-    return out
-
-
-def threshold_instance(pr, lib, route, values, kind, c):
-    e = pr.create(lib, flags=abi.CONFIG_THROUGHPUT if route == "throughput" else 0)
-    ones = np.ones((pr.K, pr.C, 4), np.float32)
-    for i, x in enumerate(values):
-        base = pr.n_tips + 2 * i * pr.n_int
-        e.set_partials(base, threshold_partials(pr, kind, c, x))
-        e.set_partials(base + 1, ones)
-    return e
-
-
 ROUTES = ["host", "device", "non_fused", "throughput", "resident"]
 
 
@@ -354,7 +219,7 @@ def test_guard_threshold(engine_lib, oracle_lib, route, kind, where):
     with threshold_instance(pr, engine_lib, route, values, kind, c) as e, \
          threshold_instance(pr, oracle_lib, route, values, kind, c) as o:
         o.set_arith(1)
-        res = run_threshold(engine_lib, e, o, route, [[threshold_spec(pr, i, kind)] for i in range(len(values))])
+        res = run_threshold(e, o, route, [[threshold_spec(pr, i, kind)] for i in range(len(values))])
         for ((le, se, lo, so),), (x, want) in zip(res, THRESHOLD_VALUES):
             assert so == want, f"oracle, x = {x:.9g}"
             assert se == want, f"x = {x:.9g}: status {se}"
@@ -378,7 +243,7 @@ def test_guard_threshold_in_one_evaluation_of_a_batch(engine_lib, oracle_lib, ro
     with threshold_instance(pr, engine_lib, route, values, kind, c) as e, \
          threshold_instance(pr, oracle_lib, route, values, kind, c) as o:
         o.set_arith(1)
-        (res,) = run_threshold(engine_lib, e, o, route, [[threshold_spec(pr, i, kind) for i in range(4)]])
+        (res,) = run_threshold(e, o, route, [[threshold_spec(pr, i, kind) for i in range(4)]])
         for i, (le, se, lo, so) in enumerate(res):
             want = abi.EVAL_UNDERFLOW if i == 2 else abi.EVAL_OK
             assert se == so == want, f"evaluation {i}"
@@ -422,7 +287,7 @@ def test_guard_flag_ignored_for_other_families(engine_lib, oracle_lib, family, S
                 res[name, tag] = (l, st)
             assert res[name, "plain"] == res[name, "flagged"], (name, res)
         assert res["engine", "plain"][1] == res["oracle", "plain"][1] == abi.EVAL_OK
-        assert rel(res["engine", "plain"][0], res["oracle", "plain"][0]) < tol_of(S)
+        assert rel(res["engine", "plain"][0], res["oracle", "plain"][0]) < lnl_tol(S)
         if family != "std":
             assert trips(o, sp, pr) == ((True, False) if trip == "rescaler" else (False, True))
         kind = {"tensor": abi.KERNEL_TENSOR, "generic": abi.KERNEL_GENERIC, "std": abi.KERNEL_STD}[family]

@@ -3,7 +3,6 @@ through a mailbox in mapped host memory, and must compute exactly what one launc
 computes.  Every comparison is bitwise."""
 from __future__ import annotations
 
-import ctypes as C
 import sys
 import time
 from pathlib import Path
@@ -13,29 +12,18 @@ import pytest
 
 sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import bench  # noqa: E402
-from mrbayes_b200 import abi, workloads  # noqa: E402
+from engine_checks import written_buffers  # noqa: E402
+from mrbayes_b200 import workloads  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
 CYCLE = 32
 
 
-def _begin_end(lib, inst, batch):
-    lnl = np.zeros(8, np.float64)
-    st = np.zeros(8, np.int32)
-    assert lib.fn("replay_begin")(inst.handle, batch) == 0
-    assert lib.fn("replay_end")(inst.handle, lnl.ctypes.data_as(C.POINTER(C.c_double)),
-                                st.ctypes.data_as(C.POINTER(C.c_int))) == 0
-    assert not st.any()
-    return lnl
-
-
 def _state(job):
     """Every partials buffer and scaler the cycle writes."""
-    inst, steps = job.insts[0], job.steps[0]
-    dests = sorted({int(op["dest"]) for s in steps for sp in s for op in sp.ops})
-    scalers = sorted({int(op["scale_write"]) for s in steps for sp in s for op in sp.ops if op["scale_write"] >= 0} |
-                     {int(sp.site_dst) for s in steps for sp in s if sp.site_dst >= 0})
+    inst = job.insts[0]
+    dests, scalers = written_buffers(job.steps[0])
     return [inst.get_partials(b) for b in dests], [inst.get_scalers(s) for s in scalers]
 
 
@@ -55,12 +43,13 @@ def _run(lib, mode, generations, pause_at=(), between=None):
                 between(g, inst)
             b = batches[g % CYCLE]
             if mode == "resident":
-                lnls.append(_begin_end(lib, inst, b))
+                inst.replay_begin(b)
+                lnl, st = inst.replay_end()
             else:
                 inst.replay(b)
                 lnl, st = inst.replay_results(b, 8)
-                assert not st.any()
-                lnls.append(lnl)
+            assert not st.any()
+            lnls.append(lnl)
         launches = inst.launch_count() - n0
         inst.synchronize()
         parts, scal = _state(job)
@@ -116,13 +105,10 @@ def test_replay_between_begin_and_end(engine_lib, launched):
         lnls = []
         for g in range(CYCLE):
             b = batches[g]
-            assert engine_lib.fn("replay_begin")(inst.handle, b) == 0
+            inst.replay_begin(b)
             if g % 4 == 1:
                 inst.replay(b)                        # the same evaluation again: same inputs, same outputs
-            lnl = np.zeros(8, np.float64)
-            st = np.zeros(8, np.int32)
-            assert engine_lib.fn("replay_end")(inst.handle, lnl.ctypes.data_as(C.POINTER(C.c_double)),
-                                               st.ctypes.data_as(C.POINTER(C.c_int))) == 0
+            lnl, st = inst.replay_end()
             assert not st.any()
             lnls.append(lnl)
     finally:

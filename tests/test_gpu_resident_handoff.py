@@ -9,7 +9,6 @@ and compares it bit for bit with one launch per generation:
     and scalers that row 7 - y wrote in generation g."""
 from __future__ import annotations
 
-import ctypes as C
 import sys
 from pathlib import Path
 
@@ -58,11 +57,8 @@ def _run(lib, mode):
         lnls = []
         for b in batches:
             if mode == "resident":
-                lnl = np.zeros(8, np.float64)
-                st = np.zeros(8, np.int32)
-                assert lib.fn("replay_begin")(inst.handle, b) == 0
-                assert lib.fn("replay_end")(inst.handle, lnl.ctypes.data_as(C.POINTER(C.c_double)),
-                                            st.ctypes.data_as(C.POINTER(C.c_int))) == 0
+                inst.replay_begin(b)
+                lnl, st = inst.replay_end()
             else:
                 inst.replay(b)
                 lnl, st = inst.replay_results(b, 8)

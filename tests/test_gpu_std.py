@@ -12,15 +12,12 @@ max_error_to_bound."""
 import numpy as np
 import pytest
 
+from engine_checks import DBL_MAX, check_with_oracle, dead_pattern_problem, evaluation_sequence, rel, tree_tol
 from f64_reference import f64_std_lnl, tree_height
-from std_problems import CASES, lanes, make_case, make_std_division, run_specs
+from std_problems import CASES, lanes, make_case, make_std_division
 from mrbayes_b200 import abi, workloads
-from test_gpu_parity import rel
-from test_gpu_paths import compare_state, dead_pattern_problem
 
 pytestmark = pytest.mark.gpu
-
-DBL_MAX = np.finfo(np.float64).max
 
 
 def smax_instantiation(S):
@@ -35,16 +32,14 @@ def check_run(engine_lib, oracle_lib, pr, supplier, record_property, updates=6):
     (caller-supplied matrices to both); every evaluation on KERNEL_STD"""
     worst, calls = 0.0, 0
     with pr.create(engine_lib) as e, pr.create(oracle_lib) as o:
-        for sp in run_specs(pr, updates, seed=3):
+        for _, sp in evaluation_sequence(pr, updates, seed=3):
             if supplier:
                 supplier(sp, [e, o])
-            (le,), (se,) = e.evaluate(sp)
-            (lo,), (so,) = o.evaluate(sp)
+            lnl, st = e.evaluate(sp)
             calls += 1
             what = f"evaluation {calls} (chain {sp.chain})"
-            assert se == so == abi.EVAL_OK, what
-            assert rel(le, lo) < 1e-9, f"{what}: engine {le!r}, oracle {lo!r}"
-            compare_state(e, o, sp, pr)
+            check_with_oracle(e, o, [sp], lnl, st, 1e-9, tree_tol(pr))
+            le = lnl[0]
             for m in sp.mats["matrix"][:3]:
                 assert np.allclose(e.get_transition_matrix(int(m)), o.get_transition_matrix(int(m)), rtol=2.5e-7,
                                    atol=1e-30), what
