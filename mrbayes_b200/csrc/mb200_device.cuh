@@ -133,6 +133,15 @@ struct ResidentJob                  // device memory, written by the leader CTA 
                                                     // JobIndexEntry pieces, each with the sequence number in .w
 };
 
+// lanes one site pattern spreads over in the 4-state and variable-state kernels, one rate category each:
+// pow2ceil(K), so that the max over a pattern's categories is an xor-shuffle
+__host__ __device__ constexpr int pattern_lanes (int K)
+{
+    int L = 1;
+    while (L < K) L <<= 1;
+    return L;
+}
+
 // chunk geometry of the 4-state kernels (shared by pack() and the kernels)
 __host__ __device__ constexpr int nuc_maxs (int K)          // P(t) slots per chunk
 {

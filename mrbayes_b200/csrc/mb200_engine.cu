@@ -18,6 +18,7 @@
 #include <time.h>
 #include <stdlib.h>
 #include <string.h>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <type_traits>
@@ -145,32 +146,60 @@ struct MatRing                         // pinned ring for caller-supplied transi
     int           next = 0;            // the slot of the next call, modulo MAT_RING
 };
 
-struct Mailbox                         // resident generation kernel (mb200_replay_begin / _end, eval_nuc4_resident_kernel)
+// The kernel family that serves an instance, fixed at creation with the tile geometry in its DevCtx
+enum class Family
 {
-    MappedArray<int4> mail;            // host -> device mailbox: MB200_RES_PIECES pieces
+    Nuc4,                              // 4 states, K <= 8: eval_nuc4_kernel and its parameter-block and resident variants
+    Tensor,                            // 61-state codons (K <= 3) and 20-state amino acids (K <= 4): eval_tcp_kernel on wgmma
+    Generic,                           // any other state count: eval_gen_kernel
+    Std                                // variable-state (STANDARD data) divisions: eval_std_kernel
+};
+
+struct Resident                        // 4-state family: the resident generation kernel (eval_nuc4_resident_kernel)
+{
+    MappedArray<int4> mail;            // host -> device mailbox: MB200_RES_PIECES pieces (allocated on first use)
     DevArray<ResidentJob> job;         // the leader CTA's copy of the current job
+    bool          ok = false;          // the kernel may serve this instance: its grid fits the device at once and
+                                       // (once tried) its mailbox could be allocated
+    bool          running = false;     // a resident kernel may still run on the stream
+    double        posted = 0.0;        // host clock (s) just before the last post
+};
+
+struct TensorQueue                     // tensor-core family: pre-split P(t) images and the node-parallel work queue
+{
+    DevArray<float> dSplit;            // pre-split (hi, lo) canonical images of every P(t)
+    DevArray<unsigned int> dCounter;   // ticket counter of the work queue (monotone)
+    unsigned int  base = 0;            // its value before the next launch's first ticket
+    DevArray<int> dFlags;              // [maxEval][numTiles + 1][flagStride] node-done flags (== launch sequence number)
+    DevArray<int> dError;
+    int           flagStride = 0;
+    int           stages = 0;          // operand-ring stages of the pipelined kernel
+    size_t        smem = 0;            // its dynamic shared memory
+};
+
+struct StdTables                       // variable-state family: mb200_set_pattern_states
+{
+    bool          ready = false;       // mb200_set_pattern_states done
+    bool          uniformMk = true;    // every matrix the engine builds is an equal-frequency Mk matrix
+    StdCtx        sx;
+    DevArray<int> dTab;                // nStates | tiIndex | bsIndex, [3][C]
+    DevArray<int2> dClasses;
+    std::vector<int> hNStates, hTiIndex, hBsIndex;
+    std::vector<size_t> hClOff;        // ragged host layout: offset of pattern c inside a category's block
 };
 
 struct Instance
 {
     Stream        stream;              // first: outlives every buffer its work may use
     mb200_instance_config cfg;
-    DevCtx        ctx;
+    Family        family = Family::Generic;
+    DevCtx        ctx;                 // geometry and buffers; a launch changes only hostSum and throughput mode's numTiles
     DevArray<uint8_t> dTip8;
     DevArray<uint64_t> dTip64;
     DevArray<int> dTipPartAmbig;
     int           seq = 0;               // launch sequence number stamped into results
-    DevArray<float> dSplit;              // tensor-core path: pre-split (hi, lo) canonical images of every P(t)
-    int           tcS = 0;               // 20 or 61 when the wgmma kernel serves this instance, else 0
     DevArray<float> dPartials, dMatrices, dScalers, dWeights;
     DevArray<double> dEigen;
-    DevArray<unsigned int> dTcCounter;   // tensor-core path: ticket counter of the node-parallel work queue (monotone)
-    unsigned int  tcBase = 0;            // its value before the next launch's first ticket
-    DevArray<int> dTcFlags;              // [maxEval][maxTiles][tcFlagStride] node-done flags (== launch sequence number)
-    DevArray<int> dTcError;
-    int           tcFlagStride = 0;
-    int           tcpStages = 0;         // pipelined tensor-core kernel: operand-ring stages that fit (0: kernel not usable)
-    size_t        tcpSmem = 0;
     DevArray<double> dFactor;            // large state counts: rank-one factors (U, W) of every eigensystem's c_ijk slices
     EigenSolver   eig;
     DevArray<uint64_t> dInvMask;
@@ -178,10 +207,10 @@ struct Instance
     DevArray<int> dTileAbort;
     DevArray<unsigned int> dTicket;
     bool          invMaskValid = false;
-    int           maxEval = 1, maxTiles = 1, numSMs = 132;
+    int           maxEval = 1, numSMs = 132;
     size_t        eigenStride = 0;     // doubles per eigen slot (all parts)
     int           cijkParts = 1;       // eigensystems per slot (one per category for NY98-type models)
-    size_t        smemGen = 0;         // dynamic smem of eval_gen_kernel
+    size_t        smemGen = 0;         // generic family: dynamic smem of eval_gen_kernel
     long long     launchKind[MB200_KERNEL_KINDS] = {0};   // per kernel family (mb200_get_kernel_launches)
     std::vector<int> tipPartAmbig;  // host copy (operand kinds of the 4-state records)
     int           tipEpoch = 0;
@@ -194,23 +223,12 @@ struct Instance
     std::vector<int> touched;          // scratch: matrices whose slotOf entry is set
     std::vector<int> dirtyOf;          // scratch: matrix index -> index in the evaluation's update list
     std::vector<DevChunk> chunkTmp; std::vector<DevMat> cmatTmp; std::vector<int> slotTmp, nChunkTmp, tipIdxTmp, writtenTmp;
-    // variable-state (STANDARD data) divisions
-    bool          std = false;         // MB200_CONFIG_VARIABLE_STATES
-    bool          stdReady = false;    // mb200_set_pattern_states done
-    bool          stdUniformMk = true; // every matrix the engine builds is an equal-frequency Mk matrix
-    StdCtx        sx;
-    DevArray<int> dStdTab;             // nStates | tiIndex | bsIndex, [3][C]
-    DevArray<int2> dStdClasses;
-    std::vector<int> hNStates, hTiIndex, hBsIndex;
-    std::vector<size_t> hClOff;        // ragged host layout: offset of pattern c inside a category's block
-    bool          timing = false;      // bracket the fused kernel with events
+    bool          timing = false;      // bracket the evaluation kernel with events
     std::vector<Event> evA, evB;       // ring of event pairs
     long long     evCount = 0;         // pairs recorded since the last read
-    Mailbox       res;
-    bool          resOk = false;       // the resident kernel may serve this instance: 4-state, its grid fits the
-                                       // device at once, and (once tried) its mailbox could be allocated
-    bool          resident = false;    // a resident kernel may still run on the stream
-    double        resPosted = 0.0;     // host clock (s) just before the last post
+    Resident      res;                 // Nuc4
+    TensorQueue   tc;                  // Tensor
+    StdTables     vs;                  // Std
 };
 
 std::mutex               gLock;
@@ -219,17 +237,45 @@ std::vector<Instance *>  gInstances;
 const int NT_GEN = 256;
 const int HOSTSUM_MAX_TILES = MB200_SEQ_SUM_TILES;   // latency path: up to this many tile partials per evaluation summed on the host
 const int NT_NUC4 = 256;                             // threads per CTA of the 4-state kernels
+const int NT_STD = 128;                              // threads per CTA of the variable-state kernel
+const int TC_MIN_ROWS = 128;                         // rows (site patterns) per tile of the tensor-core kernel = the MMA's M
 const int EV_RING = 2048;
 
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { \
     fprintf (stderr, "mb200: CUDA error %s at %s:%d (%s)\n", cudaGetErrorName (e_), __FILE__, __LINE__, cudaGetErrorString (e_)); \
     return MB200_ERROR_CUDA; } } while (0)
 
-// patterns one CTA of a 4-state kernel owns: NT threads / lanes-per-pattern (pow2ceil(K))
-int nuc4PatternsPerBlock (int K)
+Family familyOf (const mb200_instance_config &c)
 {
-    int L = (K <= 1) ? 1 : (K <= 2) ? 2 : (K <= 4) ? 4 : 8;
-    return NT_NUC4 / L;
+    const int S = c.state_count, K = c.category_count;
+    if (c.flags & MB200_CONFIG_VARIABLE_STATES) return Family::Std;
+    if (S == 4 && K <= 8) return Family::Nuc4;
+    if ((S == 61 && K <= 3) || (S == 20 && K <= 4)) return Family::Tensor;    // K > 1 at 61: omega categories (NY98 / M3)
+    return Family::Generic;
+}
+
+// Raise `kernel`'s dynamic shared-memory limit on `device` to at least `bytes`.  The limit is one per process and
+// device, and every instance there launches with it, so it only ever grows: an instance created later must not
+// take away what a live one launches with.
+std::map<std::pair<int, const void *>, int> gOptIn;       // (device, kernel) -> the largest limit set so far
+
+template <class F>
+cudaError_t optIn (F *kernel, int device, int bytes)
+{
+    std::lock_guard<std::mutex> g (gLock);
+    int &have = gOptIn[{ device, (const void *) kernel }];
+    if (bytes <= have) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute (kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) have = bytes;
+    return e;
+}
+
+// n elements in a, zeroed on the stream
+template <class A>
+int zeroed (A &a, size_t n, cudaStream_t stream)
+{
+    const int rc = a.alloc (n);
+    return rc ? rc : rcOf (cudaMemsetAsync (a, 0, n * sizeof(*a.p), stream));
 }
 
 // The 4-state kernels are compiled for K = 1..8 rate categories: calls f (std::integral_constant<int, K> ())
@@ -243,11 +289,29 @@ int withNuc4K (int K, F &&f)
 // dynamic shared memory of a 4-state kernel (the parameter-block and resident kernels take the fused layout)
 template <int K, bool FUSE> constexpr int nuc4Smem = (int) sizeof(Nuc4Smem<K, NT_NUC4, FUSE>);
 
-// The tensor-core kernels are compiled for S = 20 and 61 states: calls f (std::integral_constant<int, tcS> ())
+// The tensor-core kernels are compiled for S = 20 and 61 states: calls f (std::integral_constant<int, S> ())
 template <class F>
-auto withTcS (int tcS, F &&f)
+auto withTcS (int S, F &&f)
 {
-    return (tcS == 61) ? f (std::integral_constant<int, 61> ()) : f (std::integral_constant<int, 20> ());
+    return (S == 61) ? f (std::integral_constant<int, 61> ()) : f (std::integral_constant<int, 20> ());
+}
+
+// The variable-state kernel is compiled for padded state counts up to 4, 8, 12, 16 and 24: calls
+// f (std::integral_constant<int, SMAX> ()) with the smallest SMAX >= Sp
+template <class F>
+void withStdSmax (int Sp, F &&f)
+{
+    if (Sp <= 4)       f (std::integral_constant<int, 4> ());
+    else if (Sp <= 8)  f (std::integral_constant<int, 8> ());
+    else if (Sp <= 12) f (std::integral_constant<int, 12> ());
+    else if (Sp <= 16) f (std::integral_constant<int, 16> ());
+    else               f (std::integral_constant<int, 24> ());
+}
+
+// dynamic shared memory of tiprobs_mm_kernel (S > 32): two S x LD double matrices
+size_t mmSmem (int S)
+{
+    return (size_t)2 * S * ((S + 3) & ~3) * sizeof(double);
 }
 
 Instance *get (int id)
@@ -306,7 +370,8 @@ int validate (const Instance *I, const mb200_evaluation *evs, int count)
     const mb200_instance_config &c = I->cfg;
     if (count < 1 || count > I->maxEval)
         return MB200_ERROR_OUT_OF_RANGE;
-    if (I->std && !I->stdReady)
+    const bool isStd = (I->family == Family::Std);
+    if (isStd && !I->vs.ready)
         return MB200_ERROR_UNSUPPORTED;                 // mb200_set_pattern_states first
     for (int e = 0; e < count; e++)
         {
@@ -323,7 +388,7 @@ int validate (const Instance *I, const mb200_evaluation *evs, int count)
             {
             const mb200_matrix_update &u = ev.matrix_updates[i];
             const bool inl = (u.eigen == MB200_EIGEN_INLINE);
-            if (u.matrix < 0 || u.matrix >= c.matrix_count || (!inl && !I->std && (u.eigen < 0 || u.eigen >= c.eigen_count)))
+            if (u.matrix < 0 || u.matrix >= c.matrix_count || (!inl && !isStd && (u.eigen < 0 || u.eigen >= c.eigen_count)))
                 return MB200_ERROR_OUT_OF_RANGE;
             if (inl && (!ev.inline_eigen || c.state_count != 4))
                 return MB200_ERROR_UNSUPPORTED;
@@ -353,7 +418,7 @@ int nuc4Chunks (Instance *I, const mb200_evaluation &ev, int opOff, bool fused)
 {
     const mb200_instance_config &c = I->cfg;
     const int K = c.category_count;
-    const int maxSlots = nuc_maxs (K), maxTips = nuc_maxt (K), opc = nuc_opc (nuc4PatternsPerBlock (K));   // as in the kernel
+    const int maxSlots = nuc_maxs (K), maxTips = nuc_maxt (K), opc = nuc_opc (I->ctx.tilePatterns);   // as in the kernel
     std::vector<DevChunk> &chunks = I->chunkTmp;
     std::vector<DevMat>   &cmats = I->cmatTmp;
     std::vector<int>      &touched = I->touched;        // matrices whose slotOf entry is set (the open chunk's branches)
@@ -529,10 +594,10 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
         return rc;
     const mb200_instance_config &c = I->cfg;
     const int K = c.category_count, S = c.state_count;
-    const bool nuc4 = (S == 4 && K <= 8 && !I->std);
+    const bool nuc4 = (I->family == Family::Nuc4), tensor = (I->family == Family::Tensor);
     // state frequencies per evaluation: S, or the whole table for variable-state divisions (one vector per state count)
-    const int  nFreq = I->std ? MB200_MAX_STATES : S;
-    const long tiles = (c.pattern_count + nuc4PatternsPerBlock (K) - 1) / nuc4PatternsPerBlock (K);
+    const int  nFreq = (I->family == Family::Std) ? MB200_MAX_STATES : S;
+    const long tiles = I->ctx.patternTiles;
     // fused P(t) rebuild (every CTA rebuilds the dirty matrices of its evaluation): small launches (latency-
     // bound regime), and launches of many evaluations over few pattern tiles each (the rebuild is repeated
     // only tiles-per-evaluation times, and a second kernel + its launch gap would cost more)
@@ -566,7 +631,7 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
     size_t offCmat  = mb200_align16 (offChunk + sizeof(DevChunk) * (size_t)nExtraChunks);
     size_t offOp    = mb200_align16 (offCmat + sizeof(DevMat) * I->cmatTmp.size ());
     size_t offOrd   = mb200_align16 (offOp + sizeof(DevOp) * (size_t)nOp);      // tensor-core path: level order of the operations
-    size_t bytes    = mb200_align16 (offOrd + (I->tcS ? sizeof(int) * (size_t)nOp : 0));
+    size_t bytes    = mb200_align16 (offOrd + (tensor ? sizeof(int) * (size_t)nOp : 0));
     rc = reserveBatch (b, bytes, count);
     if (rc != MB200_SUCCESS)
         return rc;
@@ -648,7 +713,7 @@ int pack (Instance *I, Batch &b, const mb200_evaluation *evs, int count)
                 o.sw = op.scale_write; o.sr = op.scale_remove;
                 o.s1 = o.s2 = o.s3 = -1;
                 }
-            if (I->tcS)
+            if (tensor)
                 {
                 tcOrder (I, dops + oOff, ev.operation_count, dord + oOff);
                 if (ev.operation_count > b.maxOps) b.maxOps = ev.operation_count;
@@ -691,54 +756,6 @@ bool paramEligible (const Instance *I, const Batch &b)
     return b.fused && b.bytes <= (size_t) PARAM_BIG;
 }
 
-const int TC_MIN_ROWS = 128;    // rows (site patterns) per tile of the tensor-core kernel = the MMA's M
-
-// 4-state instance (at creation): opt the five launched 4-state kernels of its K in to their dynamic shared
-// memory.  The resident kernel may serve the instance if its whole grid (tiles x maxEval) fits the device at
-// once -- every CTA must be running for a job to complete; if it cannot be opted in or its occupancy cannot
-// be queried, the instance keeps its launches
-int nuc4Setup (Instance *I)
-{
-    return withNuc4K (I->cfg.category_count, [&] (auto k)
-        {
-        constexpr int KK = decltype (k)::value;
-        const cudaFuncAttribute dyn = cudaFuncAttributeMaxDynamicSharedMemorySize;
-        CK (cudaFuncSetAttribute (eval_nuc4_kernel<KK, NT_NUC4, true>, dyn, nuc4Smem<KK, true>));
-        CK (cudaFuncSetAttribute (eval_nuc4_kernel<KK, NT_NUC4, false>, dyn, nuc4Smem<KK, false>));
-        CK (cudaFuncSetAttribute (eval_nuc4_pkernel<KK, NT_NUC4, PARAM_SMALL>, dyn, nuc4Smem<KK, true>));
-        CK (cudaFuncSetAttribute (eval_nuc4_pkernel<KK, NT_NUC4, PARAM_MID>, dyn, nuc4Smem<KK, true>));
-        CK (cudaFuncSetAttribute (eval_nuc4_pkernel<KK, NT_NUC4, PARAM_BIG>, dyn, nuc4Smem<KK, true>));
-        int perSM = 0;
-        if (cudaFuncSetAttribute (eval_nuc4_resident_kernel<KK, NT_NUC4>, dyn, nuc4Smem<KK, true>) != cudaSuccess ||
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor (&perSM, eval_nuc4_resident_kernel<KK, NT_NUC4>, NT_NUC4, nuc4Smem<KK, true>) != cudaSuccess)
-            { cudaGetLastError (); perSM = 0; }
-        I->resOk = (long) perSM * I->numSMs >= (long) I->maxTiles * I->maxEval;
-        return MB200_SUCCESS;
-        });
-}
-
-// tensor-core instance of S states (at creation): the pipelined kernel gets as many operand-ring stages as
-// fit next to its static shared memory, and is opted in to the dynamic shared memory they take (tcpStages
-// stays 0 when none fits).  Returns the floats of one pre-split P(t) image.
-template <int S>
-size_t tcSetup (Instance *I)
-{
-    const int K = I->cfg.category_count;
-    int optin = 0;
-    cudaDeviceGetAttribute (&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, I->cfg.device);
-    cudaFuncAttributes fa;
-    const size_t staticBytes = (cudaFuncGetAttributes (&fa, eval_tcp_kernel<S>) == cudaSuccess) ? fa.sharedSizeBytes : 4096;    // barriers, item ring, row maxima
-    const size_t limit = ((size_t) optin > staticBytes + 1024) ? (size_t) optin - staticBytes : 0;
-    I->tcpStages = tcp_stages<S> (K, limit);
-    if (I->tcpStages > 0)
-        {
-        I->tcpSmem = I->tcpStages * tcp_stage_bytes<S> () + tcp_staging_bytes<S> (K) + tcp_tipring_bytes<S> (I->tcpStages);
-        if (cudaFuncSetAttribute (eval_tcp_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) I->tcpSmem) != cudaSuccess)
-            { cudaGetLastError (); I->tcpStages = 0; }
-        }
-    return tc_split_floats<S> ();
-}
-
 // make the evaluation just launched or posted the instance's pending one: runEnd () and retire () read
 // only this record
 void setPending (Instance *I, Batch &b, int seq, bool resident, bool hostSum, int tiles)
@@ -746,147 +763,275 @@ void setPending (Instance *I, Batch &b, int seq, bool resident, bool hostSum, in
     I->pending = { b.nEval, seq, &b, resident, hostSum, tiles };
 }
 
+// ---- per-family launch: the P(t) kernel the batch needs, then the evaluation kernel ----
+
+template <class T> const T *blobAt (const Batch &b, size_t off) { return (const T *)(b.dBlob + off); }
+
+// P(t) of the batch's matrix updates, one CTA per (update, category): above 32 states from the rank-one factors
+// (dFactor is always allocated there), writing the tensor-core family's pre-split images too when `split` is given
+int tiprobs (Instance *I, const Batch &b, const DevCtx &ctx, float *split)
+{
+    const DevEval *de = blobAt<DevEval> (b, b.offEval);
+    const double  *dd = blobAt<double> (b, b.offDbl);
+    const DevMat  *du = blobAt<DevMat> (b, b.offUpd);
+    const dim3 grid (b.nMat, ctx.K);
+    if (ctx.S > 32)
+        tiprobs_mm_kernel<<<grid, 256, mmSmem (ctx.S), I->stream>>> (ctx, de, b.nEval, dd, du, I->dFactor, split);
+    else
+        tiprobs_kernel<<<grid, 128, 0, I->stream>>> (ctx, de, b.nEval, dd, du);
+    CK (cudaGetLastError ());
+    I->launchKind[MB200_KERNEL_TIPROBS]++;
+    return MB200_SUCCESS;
+}
+
+// kernel timing brackets the evaluation kernel (and the tensor family's image split), not the P(t) kernel before it
+int timingStart (Instance *I)
+{
+    if (I->timing)
+        CK (cudaEventRecord (I->evA[I->evCount % EV_RING], I->stream));
+    return MB200_SUCCESS;
+}
+
+int launchNuc4 (Instance *I, const Batch &b, DevCtx &ctx, bool viaParams, bool toHost, DevResult *res, int seq)
+{
+    int rc = (b.nDirty > 0 && !b.fused) ? tiprobs (I, b, ctx, nullptr) : MB200_SUCCESS;
+    if (!rc) rc = timingStart (I);
+    if (rc) return rc;
+    // throughput mode (MB200_CONFIG_THROUGHPUT): several analyses share the GPU, so SM time counts, not
+    // the latency of one launch -- one CTA per evaluation walks all its tiles and builds P(t) once
+    // instead of once per tile.  Single-chunk evaluations only (per-pattern state lives in registers).
+    if (b.fused && (I->cfg.flags & MB200_CONFIG_THROUGHPUT) && b.singleChunk)
+        ctx.numTiles = 1;
+    ctx.hostSum = (toHost && b.allRoot && b.fused && ctx.numTiles <= HOSTSUM_MAX_TILES) ? 1 : 0;
+    const dim3 grid (ctx.numTiles, b.nEval);
+    const BlobOffsets off = { (int) b.offEval, (int) b.offDbl, (int) b.offUpd, (int) b.offChunk, (int) b.offCmat, (int) b.offOp };
+    const DevEval  *de = blobAt<DevEval> (b, b.offEval);
+    const double   *dd = blobAt<double> (b, b.offDbl);
+    const DevChunk *dc = blobAt<DevChunk> (b, b.offChunk);
+    const DevMat   *dm = blobAt<DevMat> (b, b.offCmat);
+    const DevOp    *dops = blobAt<DevOp> (b, b.offOp);
+    rc = withNuc4K (ctx.K, [&] (auto k)
+        {
+        constexpr int KK = decltype (k)::value;
+        // the job descriptors in the parameter block (no H2D copy); the launch copies all CAP bytes
+        auto viaBlock = [&] (auto cap)
+            {
+            constexpr int CAP = decltype (cap)::value;
+            eval_nuc4_pkernel<KK, NT_NUC4, CAP><<<grid, NT_NUC4, nuc4Smem<KK, true>, I->stream>>> (
+                ctx, off, res, seq, b.jx, *reinterpret_cast<const ParamBlob<CAP> *>(b.hBlob.p));
+            };
+        if (!viaParams && b.fused)
+            eval_nuc4_kernel<KK, NT_NUC4, true><<<grid, NT_NUC4, nuc4Smem<KK, true>, I->stream>>> (ctx, de, dd, dc, dm, dops, res, seq, b.jx);
+        else if (!viaParams)
+            eval_nuc4_kernel<KK, NT_NUC4, false><<<grid, NT_NUC4, nuc4Smem<KK, false>, I->stream>>> (ctx, de, dd, dc, dm, dops, res, seq, b.jx);
+        else if (b.bytes <= (size_t) PARAM_SMALL)
+            viaBlock (std::integral_constant<int, PARAM_SMALL> ());
+        else if (b.bytes <= (size_t) PARAM_MID)
+            viaBlock (std::integral_constant<int, PARAM_MID> ());
+        else
+            viaBlock (std::integral_constant<int, PARAM_BIG> ());
+        return MB200_SUCCESS;
+        });
+    if (rc != MB200_SUCCESS) return rc;
+    I->launchKind[MB200_KERNEL_NUC4]++;
+    return MB200_SUCCESS;
+}
+
+int launchTensor (Instance *I, const Batch &b, const DevCtx &ctx, DevResult *res, int seq)
+{
+    return withTcS (ctx.S, [&] (auto s)
+        {
+        constexpr int TS = decltype (s)::value;
+        // 61 states: tiprobs_mm_kernel writes the pre-split images of the matrices it rebuilds
+        int rc = (b.nDirty > 0) ? tiprobs (I, b, ctx, (TS == 61) ? I->tc.dSplit.p : nullptr) : MB200_SUCCESS;
+        if (!rc) rc = timingStart (I);
+        if (rc) return rc;
+        if constexpr (TS != 61)
+            if (b.nDirty > 0)
+                {
+                tc_split_kernel<TS><<<dim3 (b.nMat, ctx.K), 128, 0, I->stream>>> (I->dMatrices, I->tc.dSplit, blobAt<DevMat> (b, b.offUpd), 0, ctx.K);
+                CK (cudaGetLastError ());
+                I->launchKind[MB200_KERNEL_SETUP]++;
+                }
+        // warp-specialised pipeline over the node-parallel queue: one persistent CTA per SM
+        TcQueue Q;
+        Q.counter = I->tc.dCounter; Q.base = I->tc.base; Q.flags = I->tc.dFlags; Q.flagStride = I->tc.flagStride;
+        Q.maxOps = b.maxOps; Q.nEval = b.nEval; Q.error = I->tc.dError; Q.order = blobAt<int> (b, b.offOrd);
+        const long total = (long)(b.maxOps + 1) * b.nEval * ctx.numTiles;
+        const int  g = (int)((total < (long) I->numSMs) ? total : (long) I->numSMs);
+        I->tc.base += (unsigned int)(total + g);                  // every CTA draws exactly one ticket past the end
+        eval_tcp_kernel<TS><<<g, TCP_THREADS, I->tc.smem, I->stream>>> (ctx, Q, I->tc.stages, blobAt<DevEval> (b, b.offEval),
+                                                                       blobAt<double> (b, b.offDbl), blobAt<DevOp> (b, b.offOp), I->tc.dSplit, res, seq);
+        I->launchKind[MB200_KERNEL_TENSOR]++;
+        return MB200_SUCCESS;
+        });
+}
+
+int launchGeneric (Instance *I, const Batch &b, const DevCtx &ctx, DevResult *res, int seq)
+{
+    int rc = (b.nDirty > 0) ? tiprobs (I, b, ctx, nullptr) : MB200_SUCCESS;
+    if (!rc) rc = timingStart (I);
+    if (rc) return rc;
+    eval_gen_kernel<NT_GEN><<<dim3 (ctx.numTiles, b.nEval), NT_GEN, I->smemGen, I->stream>>> (
+        ctx, blobAt<DevEval> (b, b.offEval), blobAt<double> (b, b.offDbl), blobAt<DevOp> (b, b.offOp), res, seq);
+    I->launchKind[MB200_KERNEL_GENERIC]++;
+    return MB200_SUCCESS;
+}
+
+int launchStd (Instance *I, const Batch &b, const DevCtx &ctx, DevResult *res, int seq)
+{
+    const DevEval *de = blobAt<DevEval> (b, b.offEval);
+    const double  *dd = blobAt<double> (b, b.offDbl);
+    if (b.nDirty > 0)
+        {
+        tiprobs_std_kernel<<<b.nMat, 64, 0, I->stream>>> (ctx, I->vs.sx, de, b.nEval, dd, blobAt<DevMat> (b, b.offUpd));
+        CK (cudaGetLastError ());
+        I->launchKind[MB200_KERNEL_TIPROBS]++;
+        }
+    int rc = timingStart (I);
+    if (rc) return rc;
+    const DevOp *dops = blobAt<DevOp> (b, b.offOp);
+    const int mk = I->vs.uniformMk ? 1 : 0;
+    withStdSmax (ctx.Sp, [&] (auto smax)
+        {
+        eval_std_kernel<decltype (smax)::value, NT_STD><<<dim3 (ctx.numTiles, b.nEval), NT_STD, 0, I->stream>>> (
+            ctx, I->vs.sx, de, dd, dops, res, seq, mk);
+        });
+    I->launchKind[MB200_KERNEL_STD]++;
+    return MB200_SUCCESS;
+}
+
 // launch the evaluation of a packed batch.  viaParams: the job lives in b.hBlob only and rides in the
 // parameter block (otherwise the caller has copied it to dBlob).  toHost: the results go to the batch's
 // mapped host buffer and the launch becomes the pending evaluation; else they go to b.dRes.
 int launch (Instance *I, Batch &b, bool viaParams, bool toHost)
 {
-    const DevEval  *de = (const DevEval  *)(b.dBlob + b.offEval);
-    const double   *dd = (const double   *)(b.dBlob + b.offDbl);
-    const DevMat   *du = (const DevMat   *)(b.dBlob + b.offUpd);
-    const DevChunk *dc = (const DevChunk *)(b.dBlob + b.offChunk);
-    const DevMat   *dm = (const DevMat   *)(b.dBlob + b.offCmat);
-    const DevOp    *dops = (const DevOp  *)(b.dBlob + b.offOp);
     DevResult *res = toHost ? b.hRes.dev : b.dRes;
     DevCtx ctx = I->ctx;
     const int seq = ++I->seq;
-
-    if (b.needInv)
+    int rc = b.needInv ? ensureInvMask (I) : MB200_SUCCESS;
+    if (rc != MB200_SUCCESS) return rc;
+    switch (I->family)
         {
-        int rc = ensureInvMask (I);
-        if (rc != MB200_SUCCESS) return rc;
+        case Family::Nuc4:    rc = launchNuc4 (I, b, ctx, viaParams, toHost, res, seq); break;
+        case Family::Tensor:  rc = launchTensor (I, b, ctx, res, seq); break;
+        case Family::Generic: rc = launchGeneric (I, b, ctx, res, seq); break;
+        case Family::Std:     rc = launchStd (I, b, ctx, res, seq); break;
         }
-    if (b.nDirty > 0 && I->std)
-        {
-        tiprobs_std_kernel<<<b.nMat, 64, 0, I->stream>>> (ctx, I->sx, de, b.nEval, dd, du);
-        CK (cudaGetLastError ());
-        I->launchKind[MB200_KERNEL_TIPROBS]++;
-        }
-    else if (b.nDirty > 0 && !b.fused)
-        {
-        if (ctx.S > 32)             // dFactor is always allocated for these state counts
-            {
-            dim3 grid (b.nMat, ctx.K);
-            const int LD = (ctx.S + 3) & ~3;
-            tiprobs_mm_kernel<<<grid, 256, (size_t)2 * ctx.S * LD * sizeof(double), I->stream>>> (ctx, de, b.nEval, dd, du, I->dFactor,
-                                                                                                   (I->tcS == 61) ? I->dSplit.p : nullptr);
-            }
-        else
-            {
-            dim3 grid (b.nMat, ctx.K);
-            tiprobs_kernel<<<grid, 128, 0, I->stream>>> (ctx, de, b.nEval, dd, du);
-            }
-        CK (cudaGetLastError ());
-        I->launchKind[MB200_KERNEL_TIPROBS]++;
-        }
-    const int evSlot = (int)(I->evCount % EV_RING);
-    if (I->timing)
-        CK (cudaEventRecord (I->evA[evSlot], I->stream));
-    if (I->std)
-        {
-        const int NT = 128;
-        ctx.tilePatterns = NT / I->sx.lanes;
-        ctx.numTiles = (ctx.C + ctx.tilePatterns - 1) / ctx.tilePatterns;
-        dim3 grid (ctx.numTiles, b.nEval);
-        const int mk = I->stdUniformMk ? 1 : 0;
-        if (ctx.Sp <= 4)       eval_std_kernel<4, 128><<<grid, NT, 0, I->stream>>> (ctx, I->sx, de, dd, dops, res, seq, mk);
-        else if (ctx.Sp <= 8)  eval_std_kernel<8, 128><<<grid, NT, 0, I->stream>>> (ctx, I->sx, de, dd, dops, res, seq, mk);
-        else if (ctx.Sp <= 12) eval_std_kernel<12, 128><<<grid, NT, 0, I->stream>>> (ctx, I->sx, de, dd, dops, res, seq, mk);
-        else if (ctx.Sp <= 16) eval_std_kernel<16, 128><<<grid, NT, 0, I->stream>>> (ctx, I->sx, de, dd, dops, res, seq, mk);
-        else                   eval_std_kernel<24, 128><<<grid, NT, 0, I->stream>>> (ctx, I->sx, de, dd, dops, res, seq, mk);
-        I->launchKind[MB200_KERNEL_STD]++;
-        }
-    else if (ctx.S == 4 && ctx.K <= 8)
-        {
-        ctx.tilePatterns = nuc4PatternsPerBlock (ctx.K);
-        ctx.patternTiles = (ctx.C + ctx.tilePatterns - 1) / ctx.tilePatterns;
-        ctx.numTiles = ctx.patternTiles;
-        // throughput mode (MB200_CONFIG_THROUGHPUT): several analyses share the GPU, so SM time counts, not
-        // the latency of one launch -- one CTA per evaluation walks all its tiles and builds P(t) once
-        // instead of once per tile.  Single-chunk evaluations only (per-pattern state lives in registers).
-        if (b.fused && (I->cfg.flags & MB200_CONFIG_THROUGHPUT) && b.singleChunk)
-            ctx.numTiles = 1;
-        ctx.hostSum = (toHost && b.allRoot && b.fused && ctx.numTiles <= HOSTSUM_MAX_TILES) ? 1 : 0;
-        const dim3 grid (ctx.numTiles, b.nEval);
-        const BlobOffsets off = { (int) b.offEval, (int) b.offDbl, (int) b.offUpd, (int) b.offChunk, (int) b.offCmat, (int) b.offOp };
-        int rc = withNuc4K (ctx.K, [&] (auto k)
-            {
-            constexpr int KK = decltype (k)::value;
-            // the job descriptors in the parameter block (no H2D copy); the launch copies all CAP bytes
-            auto viaBlock = [&] (auto cap)
-                {
-                constexpr int CAP = decltype (cap)::value;
-                eval_nuc4_pkernel<KK, NT_NUC4, CAP><<<grid, NT_NUC4, nuc4Smem<KK, true>, I->stream>>> (
-                    ctx, off, res, seq, b.jx, *reinterpret_cast<const ParamBlob<CAP> *>(b.hBlob.p));
-                };
-            if (!viaParams && b.fused)
-                eval_nuc4_kernel<KK, NT_NUC4, true><<<grid, NT_NUC4, nuc4Smem<KK, true>, I->stream>>> (ctx, de, dd, dc, dm, dops, res, seq, b.jx);
-            else if (!viaParams)
-                eval_nuc4_kernel<KK, NT_NUC4, false><<<grid, NT_NUC4, nuc4Smem<KK, false>, I->stream>>> (ctx, de, dd, dc, dm, dops, res, seq, b.jx);
-            else if (b.bytes <= (size_t) PARAM_SMALL)
-                viaBlock (std::integral_constant<int, PARAM_SMALL> ());
-            else if (b.bytes <= (size_t) PARAM_MID)
-                viaBlock (std::integral_constant<int, PARAM_MID> ());
-            else
-                viaBlock (std::integral_constant<int, PARAM_BIG> ());
-            return MB200_SUCCESS;
-            });
-        if (rc != MB200_SUCCESS) return rc;
-        I->launchKind[MB200_KERNEL_NUC4]++;
-        }
-    else if (I->tcS)
-        {
-        ctx.tilePatterns = 128;
-        ctx.numTiles = (ctx.C + 127) / 128;
-        int rc = withTcS (I->tcS, [&] (auto s)
-            {
-            constexpr int TS = decltype (s)::value;
-            // refresh the pre-split images of the matrices just rebuilt (61 states: tiprobs_mm_kernel has
-            // written them already)
-            if constexpr (TS != 61)
-                if (b.nDirty > 0)
-                    {
-                    tc_split_kernel<TS><<<dim3 (b.nMat, ctx.K), 128, 0, I->stream>>> (I->dMatrices, I->dSplit, du, 0, ctx.K);
-                    CK (cudaGetLastError ());
-                    I->launchKind[MB200_KERNEL_SETUP]++;
-                    }
-            // warp-specialised pipeline over the node-parallel queue: one persistent CTA per SM
-            TcQueue Q;
-            Q.counter = I->dTcCounter; Q.base = I->tcBase; Q.flags = I->dTcFlags; Q.flagStride = I->tcFlagStride;
-            Q.maxOps = b.maxOps; Q.nEval = b.nEval; Q.error = I->dTcError; Q.order = (const int *)(b.dBlob + b.offOrd);
-            const long total = (long)(b.maxOps + 1) * b.nEval * ctx.numTiles;
-            const int  g = (int)((total < (long) I->numSMs) ? total : (long) I->numSMs);
-            I->tcBase += (unsigned int)(total + g);                  // every CTA draws exactly one ticket past the end
-            eval_tcp_kernel<TS><<<g, TCP_THREADS, I->tcpSmem, I->stream>>> (ctx, Q, I->tcpStages, de, dd, dops, I->dSplit, res, seq);
-            return MB200_SUCCESS;
-            });
-        if (rc != MB200_SUCCESS) return rc;
-        I->launchKind[MB200_KERNEL_TENSOR]++;
-        }
-    else
-        {
-        eval_gen_kernel<NT_GEN><<<dim3 (ctx.numTiles, b.nEval), NT_GEN, I->smemGen, I->stream>>> (ctx, de, dd, dops, res, seq);
-        I->launchKind[MB200_KERNEL_GENERIC]++;
-        }
+    if (rc != MB200_SUCCESS) return rc;
     CK (cudaGetLastError ());
     if (I->timing)
         {
-        CK (cudaEventRecord (I->evB[evSlot], I->stream));
+        CK (cudaEventRecord (I->evB[I->evCount % EV_RING], I->stream));
         I->evCount++;
         }
     if (toHost)
         setPending (I, b, seq, false, ctx.hostSum != 0, ctx.numTiles);
     return MB200_SUCCESS;
+}
+
+// ---- per-family setup (at creation): tile geometry into I->ctx, the dynamic shared memory of the kernels the
+// family launches, family-only buffers
+
+// 4-state instance: tiles of NT_NUC4 / pattern_lanes (K) patterns; the five launched 4-state kernels of its K are
+// opted in to their dynamic shared memory.  The resident kernel may serve the instance if its whole grid (tiles x
+// maxEval) fits the device at once -- every CTA must be running for a job to complete; if it cannot be opted in or
+// its occupancy cannot be queried, the instance keeps its launches
+int nuc4Setup (Instance *I)
+{
+    DevCtx &x = I->ctx;
+    x.tilePatterns = NT_NUC4 / pattern_lanes (x.K);
+    x.patternTiles = x.numTiles = (x.C + x.tilePatterns - 1) / x.tilePatterns;
+    return withNuc4K (x.K, [&] (auto k)
+        {
+        constexpr int KK = decltype (k)::value;
+        const int dev = I->cfg.device;
+        CK (optIn (eval_nuc4_kernel<KK, NT_NUC4, true>, dev, nuc4Smem<KK, true>));
+        CK (optIn (eval_nuc4_kernel<KK, NT_NUC4, false>, dev, nuc4Smem<KK, false>));
+        CK (optIn (eval_nuc4_pkernel<KK, NT_NUC4, PARAM_SMALL>, dev, nuc4Smem<KK, true>));
+        CK (optIn (eval_nuc4_pkernel<KK, NT_NUC4, PARAM_MID>, dev, nuc4Smem<KK, true>));
+        CK (optIn (eval_nuc4_pkernel<KK, NT_NUC4, PARAM_BIG>, dev, nuc4Smem<KK, true>));
+        int perSM = 0;
+        if (optIn (eval_nuc4_resident_kernel<KK, NT_NUC4>, dev, nuc4Smem<KK, true>) != cudaSuccess ||
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor (&perSM, eval_nuc4_resident_kernel<KK, NT_NUC4>, NT_NUC4, nuc4Smem<KK, true>) != cudaSuccess)
+            { cudaGetLastError (); perSM = 0; }
+        I->res.ok = (long) perSM * I->numSMs >= (long) x.numTiles * I->maxEval;
+        return MB200_SUCCESS;
+        });
+}
+
+// the pipelined tensor-core kernel of S states gets as many operand-ring stages as fit next to its static shared
+// memory, and is opted in to the dynamic shared memory they take (stages stays 0 when none fits, or the opt-in is
+// refused).  Returns the floats of one pre-split P(t) image.
+template <int S>
+size_t tcStages (Instance *I)
+{
+    const int K = I->cfg.category_count;
+    int optin = 0;
+    cudaDeviceGetAttribute (&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, I->cfg.device);
+    cudaFuncAttributes fa;
+    const size_t staticBytes = (cudaFuncGetAttributes (&fa, eval_tcp_kernel<S>) == cudaSuccess) ? fa.sharedSizeBytes : 4096;    // barriers, item ring, row maxima
+    const size_t limit = ((size_t) optin > staticBytes + 1024) ? (size_t) optin - staticBytes : 0;
+    I->tc.stages = tcp_stages<S> (K, limit);
+    if (I->tc.stages > 0)
+        {
+        I->tc.smem = I->tc.stages * tcp_stage_bytes<S> () + tcp_staging_bytes<S> (K) + tcp_tipring_bytes<S> (I->tc.stages);
+        if (optIn (eval_tcp_kernel<S>, I->cfg.device, (int) I->tc.smem) != cudaSuccess)
+            { cudaGetLastError (); I->tc.stages = 0; }
+        }
+    return tc_split_floats<S> ();
+}
+
+// tensor-core instance: tiles of TC_MIN_ROWS patterns, one persistent CTA per SM; 61 states also opt in
+// tiprobs_mm_kernel, which writes the pre-split images
+int tensorSetup (Instance *I)
+{
+    const mb200_instance_config &c = I->cfg;
+    DevCtx &x = I->ctx;
+    x.tilePatterns = TC_MIN_ROWS;
+    x.numTiles = (x.C + TC_MIN_ROWS - 1) / TC_MIN_ROWS;
+    int rc = (x.S > 32) ? rcOf (optIn (tiprobs_mm_kernel, c.device, (int) mmSmem (x.S))) : MB200_SUCCESS;
+    if (rc) return rc;
+    const size_t fl = withTcS (x.S, [&] (auto s) { return tcStages<decltype (s)::value> (I); });
+    if (!I->tc.stages) return MB200_ERROR_UNSUPPORTED;          // not for K <= 4 on a 227 KB part
+    I->tc.flagStride = (c.partials_count - c.tip_count) + 1;
+    rc = zeroed (I->tc.dSplit, (size_t)c.matrix_count * x.K * fl, I->stream);
+    if (!rc) rc = zeroed (I->tc.dCounter, 1, I->stream);
+    if (!rc) rc = zeroed (I->tc.dError, 1, I->stream);
+    if (!rc) rc = zeroed (I->tc.dFlags, (size_t) I->maxEval * (x.numTiles + 1) * I->tc.flagStride, I->stream);
+    return rc;
+}
+
+// generic instance: TP patterns per tile and KB rate categories per pass of eval_gen_kernel
+int genericSetup (Instance *I)
+{
+    DevCtx &x = I->ctx;
+    const int S = x.S, Sp = x.Sp, K = x.K, C = x.C;
+    // keep P + child tile + product under ~96 KB
+    int TP = 32;
+    // rate categories per pass: all of them when their P matrices fit in 48 KB, else one at a time
+    const int KB = ((size_t)K * S * (S + 1) * sizeof(float) <= 48*1024) ? K : 1;
+    auto smemFor = [&] (int tp) { return sizeof(float) * ((size_t)KB*S*(S+1) + (size_t)KB*tp*(Sp+1) + (size_t)K*tp*S + 3*(size_t)tp); };
+    while (TP > 1 && smemFor (TP) > 96*1024) TP >>= 1;
+    // small divisions: a CTA walks its tile's nodes one (child, category) step at a time, each step a global round trip and
+    // two barriers whatever the tile holds -- fewer patterns per tile put more SMs on the evaluation
+    while (TP > 4 && (C + TP - 1) / TP < I->numSMs) TP >>= 1;
+    I->smemGen = smemFor (TP);
+    x.tilePatterns = TP;
+    x.genKB = KB;
+    x.numTiles = (C + TP - 1) / TP;
+    int rc = (S > 32) ? rcOf (optIn (tiprobs_mm_kernel, I->cfg.device, (int) mmSmem (S))) : MB200_SUCCESS;
+    if (!rc && I->smemGen > 48*1024) rc = rcOf (optIn (eval_gen_kernel<NT_GEN>, I->cfg.device, (int) I->smemGen));
+    return rc;
+}
+
+// variable-state instance: tiles of NT_STD / pattern_lanes (K) patterns
+void stdSetup (Instance *I)
+{
+    DevCtx &x = I->ctx;
+    I->vs.sx.lanes = pattern_lanes (x.K);
+    x.tilePatterns = NT_STD / I->vs.sx.lanes;
+    x.numTiles = (x.C + x.tilePatterns - 1) / x.tilePatterns;
 }
 
 // ---- resident generation kernel (eval_nuc4_resident_kernel) ----------------------------------
@@ -929,16 +1074,6 @@ void post (Instance *I, int seq, int count, const Batch *b)
     __atomic_signal_fence (__ATOMIC_SEQ_CST);
 }
 
-DevCtx residentCtx (const Instance *I)
-{
-    DevCtx ctx = I->ctx;
-    ctx.tilePatterns = nuc4PatternsPerBlock (ctx.K);
-    ctx.patternTiles = (ctx.C + ctx.tilePatterns - 1) / ctx.tilePatterns;
-    ctx.numTiles = ctx.patternTiles;
-    ctx.hostSum = 1;
-    return ctx;
-}
-
 // Which batches the resident kernel serves: fused 4-state batches whose evaluations all reach the root,
 // whose tile partials the host sums and whose job index covers every evaluation -- and only while this
 // instance is the only one on its device, so that idle resident CTAs never hold SMs other analyses
@@ -947,10 +1082,10 @@ DevCtx residentCtx (const Instance *I)
 bool residentEligible (Instance *I, const Batch &b)
 {
     const mb200_instance_config &c = I->cfg;
-    if (!I->resOk || I->timing || (c.flags & MB200_CONFIG_THROUGHPUT) || !b.fused || !b.allRoot ||
+    if (I->family != Family::Nuc4 || !I->res.ok || I->timing || (c.flags & MB200_CONFIG_THROUGHPUT) || !b.fused || !b.allRoot ||
         b.nEval > MB200_JOB_INDEX_MAX || b.jx.n != b.nEval || I->maxEval > MB200_JOB_INDEX_MAX)
         return false;
-    if (residentCtx (I).numTiles > HOSTSUM_MAX_TILES)
+    if (I->ctx.numTiles > HOSTSUM_MAX_TILES)
         return false;
     {
     std::lock_guard<std::mutex> g (gLock);
@@ -963,11 +1098,11 @@ bool residentEligible (Instance *I, const Batch &b)
     if (!I->res.job)
         {
         // mailbox and job copy on first use; without them the instance keeps its launches
-        Mailbox m;
-        if (m.mail.alloc (MB200_RES_PIECES) || m.job.alloc (1) || rcOf (cudaMemset (m.job, 0, sizeof(ResidentJob))))
-            { I->resOk = false; return false; }
-        memset (m.mail, 0, sizeof(int4) * MB200_RES_PIECES);
-        I->res = std::move (m);
+        MappedArray<int4> mail; DevArray<ResidentJob> job;
+        if (mail.alloc (MB200_RES_PIECES) || job.alloc (1) || rcOf (cudaMemset (job, 0, sizeof(ResidentJob))))
+            { I->res.ok = false; return false; }
+        memset (mail, 0, sizeof(int4) * MB200_RES_PIECES);
+        I->res.mail = std::move (mail); I->res.job = std::move (job);
         }
     return true;
 }
@@ -982,15 +1117,16 @@ int residentStart (Instance *I, Batch &b)
         if (rc != MB200_SUCCESS) return rc;
         }
     // past half the idle timeout the kernel may have exited: a cheap check saves a lost post
-    if (I->resident && wallNow () - I->resPosted > 0.5e-9 * (double) RES_IDLE_NS && cudaStreamQuery (I->stream) == cudaSuccess)
-        I->resident = false;
-    const DevCtx ctx = residentCtx (I);
+    if (I->res.running && wallNow () - I->res.posted > 0.5e-9 * (double) RES_IDLE_NS && cudaStreamQuery (I->stream) == cudaSuccess)
+        I->res.running = false;
+    DevCtx ctx = I->ctx;
+    ctx.hostSum = 1;
     // a new kernel starts past every sequence number an earlier kernel may have left in its job copy
-    const int seq0 = I->resident ? 0 : ++I->seq;
+    const int seq0 = I->res.running ? 0 : ++I->seq;
     const int seq = ++I->seq;
-    I->resPosted = wallNow ();
+    I->res.posted = wallNow ();
     post (I, seq, b.nEval, &b);
-    if (!I->resident)
+    if (!I->res.running)
         {
         const dim3 grid (ctx.numTiles, I->maxEval);
         int rc = withNuc4K (ctx.K, [&] (auto k)
@@ -1001,7 +1137,7 @@ int residentStart (Instance *I, Batch &b)
             return MB200_SUCCESS;
             });
         if (rc != MB200_SUCCESS) return rc;
-        I->resident = true;
+        I->res.running = true;
         I->launchKind[MB200_KERNEL_NUC4]++;
         }
     setPending (I, b, seq, true, true, ctx.numTiles);
@@ -1027,13 +1163,13 @@ int waitResults (Instance *I)
 #if defined(__x86_64__)
             __builtin_ia32_pause ();
 #endif
-            if ((++spins & (I->resident ? 0x3fffu : 0xfffffu)) == 0)
+            if ((++spins & (I->res.running ? 0x3fffu : 0xfffffu)) == 0)
                 {
                 cudaError_t q = cudaStreamQuery (I->stream);
                 if (q == cudaSuccess)
                     {
                     if (r[e].seq == p.seq) break;
-                    if (I->resident && p.resident)
+                    if (I->res.running && p.resident)
                         {
                         for (int i = 0; i < slots; i++)
                             if (r[i].seq == p.seq)
@@ -1041,7 +1177,7 @@ int waitResults (Instance *I)
                                 fprintf (stderr, "mb200: resident kernel exited in the middle of a job\n");
                                 return MB200_ERROR_GENERAL;
                                 }
-                        I->resident = false;
+                        I->res.running = false;
                         int rc = residentStart (I, *p.batch);
                         if (rc != MB200_SUCCESS) return rc;
                         e = -1;                 // every slot again, for the new sequence number
@@ -1055,7 +1191,7 @@ int waitResults (Instance *I)
                     fprintf (stderr, "mb200: CUDA error %s while waiting for results\n", cudaGetErrorName (q));
                     return MB200_ERROR_CUDA;
                     }
-                else if (I->resident && wallNow () - t0 > RES_DEADLINE_S)
+                else if (I->res.running && wallNow () - t0 > RES_DEADLINE_S)
                     {
                     fprintf (stderr, "mb200: no results from the resident kernel within %.0f s\n", RES_DEADLINE_S);
                     return MB200_ERROR_GENERAL;
@@ -1072,14 +1208,14 @@ int waitResults (Instance *I)
 // so that the stop does not overwrite a post the leader has not taken yet
 int retire (Instance *I)
 {
-    if (!I->resident)
+    if (!I->res.running)
         return MB200_SUCCESS;
     if (I->pending.count > 0 && I->pending.resident)
         {
         int rc = waitResults (I);
         if (rc != MB200_SUCCESS) return rc;
         }
-    I->resident = false;
+    I->res.running = false;
     post (I, ++I->seq, MB200_RES_STOP, nullptr);
     CK (cudaStreamSynchronize (I->stream));     // bounded: the leader takes the stop within microseconds, or has exited
     return MB200_SUCCESS;
@@ -1172,7 +1308,7 @@ int makeEigenSolver (const Instance *I, EigenSolver &out)
     if (!rc) rc = g.log.alloc ((size_t)parts * MB200_EIG_LOG_DOUBLES / 2);
     if (!rc) rc = g.rounds.alloc (parts);
     if (!rc) rc = makeEvents (g.evIn, slots, cudaEventDisableTiming);
-    if (!rc) rc = rcOf (cudaFuncSetAttribute (eigen_rotations_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) eigen_smem_bytes ()));
+    if (!rc) rc = rcOf (optIn (eigen_rotations_kernel, I->cfg.device, (int) eigen_smem_bytes ()));
     if (rc != MB200_SUCCESS) return rc;
     *g.status.p = 0;
     g.warmChain.assign (slots, -1);
@@ -1250,6 +1386,7 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
 
     Instance *I = new Instance ();
     I->cfg = *cfg;
+    I->family = familyOf (*cfg);
     I->numSMs = sms > 0 ? sms : 132;
     I->maxEval = cfg->max_evaluations > 0 ? cfg->max_evaluations : 1;
     const int S = cfg->state_count, K = cfg->category_count, C = cfg->pattern_count;
@@ -1258,89 +1395,47 @@ int mb200_create_instance (const mb200_instance_config *cfg, int *instance)
     I->cijkParts = ((cfg->flags >> 8) & 0xff) > 1 ? ((cfg->flags >> 8) & 0xff) : 1;
     if (I->cijkParts != 1 && (I->cijkParts != K || S == 4)) { delete I; return MB200_ERROR_UNSUPPORTED; }
     I->eigenStride = (size_t) I->cijkParts * (2*(size_t)S + (size_t)S*S*S);
-
-    // tile geometry of the generic kernel: keep P + child tile + product under ~96 KB
-    int TP = 32;
-    // rate categories per pass: all of them when their P matrices fit in 48 KB, else one at a time
-    const int KB = ((size_t)K * S * (S + 1) * sizeof(float) <= 48*1024) ? K : 1;
-    auto smemFor = [&] (int tp) { return sizeof(float) * ((size_t)KB*S*(S+1) + (size_t)KB*tp*(Sp+1) + (size_t)K*tp*S + 3*(size_t)tp); };
-    while (TP > 1 && smemFor (TP) > 96*1024) TP >>= 1;
-    // small divisions: a CTA walks its tile's nodes one (child, category) step at a time, each step a global round trip and
-    // two barriers whatever the tile holds -- fewer patterns per tile put more SMs on the evaluation
-    while (TP > 4 && (C + TP - 1) / TP < I->numSMs) TP >>= 1;
-    I->smemGen = smemFor (TP);
-    I->std = (cfg->flags & MB200_CONFIG_VARIABLE_STATES) != 0;
-    if (I->std && (S > MB200_STD_MAX_STATES || I->cijkParts != 1)) { delete I; return MB200_ERROR_UNSUPPORTED; }
-    const bool nuc4 = (S == 4 && K <= 8 && !I->std);
-    if (nuc4 && (nInt * K * C >= (1ull << 32) || (size_t)cfg->tip_count * C >= (1ull << 32)))
+    if (I->family == Family::Std && (S > MB200_STD_MAX_STATES || I->cijkParts != 1)) { delete I; return MB200_ERROR_UNSUPPORTED; }
+    if (I->family == Family::Nuc4 && (nInt * K * C >= (1ull << 32) || (size_t)cfg->tip_count * C >= (1ull << 32)))
         { delete I; return MB200_ERROR_OUT_OF_RANGE; }      // 4-state records carry 32-bit element offsets (64 GB of partials)
-    if (!I->std)
-        {
-        if (S == 61 && K <= 3) I->tcS = 61;      // 61-state codon (K > 1: omega categories, NY98 / M3), wgmma path
-        if (S == 20 && K <= 4) I->tcS = 20;      // 20-state amino acids, wgmma path
-        }
-    int stdLanes = 1;
-    while (stdLanes < K) stdLanes <<= 1;
-    if (I->std)
-        I->maxTiles = (C + 128 / stdLanes - 1) / (128 / stdLanes);
-    else
-    I->maxTiles = I->tcS ? (C + TC_MIN_ROWS - 1) / TC_MIN_ROWS + 1 : nuc4 ? (C + nuc4PatternsPerBlock (K) - 1) / nuc4PatternsPerBlock (K) : (C + TP - 1) / TP;
-
-    // n elements of a, zeroed on the stream
-    auto make = [&] (auto &a, size_t n) { int r = a.alloc (n); return r ? r : rcOf (cudaMemsetAsync (a, 0, n * sizeof(*a.p), I->stream)); };
-    int rc = rcOf (cudaStreamCreateWithFlags (&I->stream.h, cudaStreamNonBlocking));
-    if (!rc) rc = make (I->dTip8,     (size_t)cfg->tip_count * C);
-    if (!rc) rc = make (I->dTip64,    (size_t)cfg->tip_count * C);
-    if (!rc) rc = make (I->dTipPartAmbig, (size_t)cfg->tip_count);
-    if (!rc) rc = make (I->dPartials, nInt * K * C * Sp);
-    if (!rc) rc = make (I->dMatrices, (size_t)cfg->matrix_count * K * S * S);
-    if (!rc) rc = make (I->dScalers,  (size_t)cfg->scaler_count * C);
-    if (!rc) rc = make (I->dWeights,  (size_t)cfg->weight_rows * C);
-    if (!rc) rc = make (I->dEigen,    (size_t)cfg->eigen_count * I->eigenStride);
-    if (!rc && S > 32)
-        {
-        rc = make (I->dFactor, (size_t)cfg->eigen_count * I->cijkParts * 2 * S * S);
-        const int LD = (S + 3) & ~3;
-        if (!rc) rc = rcOf (cudaFuncSetAttribute (tiprobs_mm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)2 * S * LD * sizeof(double))));
-        }
-    if (!rc && I->tcS)
-        {
-        // warp-specialised pipelined kernel: one CTA per SM, as many operand-ring stages as fit
-        const size_t fl = withTcS (I->tcS, [&] (auto s) { return tcSetup<decltype (s)::value> (I); });
-        I->tcFlagStride = (int) nInt + 1;
-        const size_t nFlags = (size_t) I->maxEval * ((size_t)(C + TC_MIN_ROWS - 1) / TC_MIN_ROWS + 1) * I->tcFlagStride;
-        rc = I->tcpStages ? make (I->dSplit, (size_t)cfg->matrix_count * K * fl) : MB200_ERROR_UNSUPPORTED;  // 0 stages: not for K <= 4 on a 227 KB part
-        if (!rc) rc = make (I->dTcCounter, 1);
-        if (!rc) rc = make (I->dTcError, 1);
-        if (!rc) rc = make (I->dTcFlags, nFlags);
-        }
-    if (!rc) rc = make (I->dInvMask,  (size_t)C);
-    if (!rc) rc = make (I->dTilePartial, (size_t)I->maxEval * I->maxTiles);
-    if (!rc) rc = make (I->dTileAbort,   (size_t)I->maxEval * I->maxTiles);
-    if (!rc) rc = make (I->dTicket,      (size_t)I->maxEval);
-    if (!rc && I->smemGen > 48*1024) rc = rcOf (cudaFuncSetAttribute (eval_gen_kernel<NT_GEN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) I->smemGen));
-    if (!rc && nuc4 && nuc4Setup (I)) rc = MB200_ERROR_CUDA;
-    if (!rc) rc = rcOf (cudaStreamSynchronize (I->stream));
-    if (rc != MB200_SUCCESS)
-        { destroy (I); return rc; }           // the half-built instance frees what it holds
-    if (I->std)
-        {
-        memset (&I->sx, 0, sizeof(I->sx));
-        I->sx.lanes = stdLanes;
-        }
-    I->tipPartAmbig.assign (cfg->tip_count, 0);
 
     DevCtx &x = I->ctx;
     memset (&x, 0, sizeof(x));
     x.S = S; x.Sp = Sp; x.K = K; x.C = C;
     x.tipCount = cfg->tip_count; x.partialsCount = cfg->partials_count; x.matrixCount = cfg->matrix_count;
     x.scalerCount = cfg->scaler_count; x.eigenCount = cfg->eigen_count; x.weightRows = cfg->weight_rows;
-    x.tilePatterns = I->tcS ? 128 : nuc4 ? nuc4PatternsPerBlock (K) : TP;
-    x.genKB = KB;
-    x.numTiles = I->maxTiles;
+    x.cijkParts = I->cijkParts;
+
+    int rc = rcOf (cudaStreamCreateWithFlags (&I->stream.h, cudaStreamNonBlocking));
+    if (!rc && S > 32) rc = zeroed (I->dFactor, (size_t)cfg->eigen_count * I->cijkParts * 2 * S * S, I->stream);
+    if (!rc)
+        switch (I->family)
+            {
+            case Family::Nuc4:    rc = nuc4Setup (I); break;
+            case Family::Tensor:  rc = tensorSetup (I); break;
+            case Family::Generic: rc = genericSetup (I); break;
+            case Family::Std:     stdSetup (I); break;
+            }
+    // tile partials per evaluation: the tensor family's buffers, like its flags, hold one tile more than its kernel uses
+    const size_t tileSlots = (size_t) I->maxEval * (x.numTiles + (I->family == Family::Tensor ? 1 : 0));
+    if (!rc) rc = zeroed (I->dTip8,     (size_t)cfg->tip_count * C, I->stream);
+    if (!rc) rc = zeroed (I->dTip64,    (size_t)cfg->tip_count * C, I->stream);
+    if (!rc) rc = zeroed (I->dTipPartAmbig, (size_t)cfg->tip_count, I->stream);
+    if (!rc) rc = zeroed (I->dPartials, nInt * K * C * Sp, I->stream);
+    if (!rc) rc = zeroed (I->dMatrices, (size_t)cfg->matrix_count * K * S * S, I->stream);
+    if (!rc) rc = zeroed (I->dScalers,  (size_t)cfg->scaler_count * C, I->stream);
+    if (!rc) rc = zeroed (I->dWeights,  (size_t)cfg->weight_rows * C, I->stream);
+    if (!rc) rc = zeroed (I->dEigen,    (size_t)cfg->eigen_count * I->eigenStride, I->stream);
+    if (!rc) rc = zeroed (I->dInvMask,  (size_t)C, I->stream);
+    if (!rc) rc = zeroed (I->dTilePartial, tileSlots, I->stream);
+    if (!rc) rc = zeroed (I->dTileAbort,   tileSlots, I->stream);
+    if (!rc) rc = zeroed (I->dTicket,      (size_t)I->maxEval, I->stream);
+    if (!rc) rc = rcOf (cudaStreamSynchronize (I->stream));
+    if (rc != MB200_SUCCESS)
+        { destroy (I); return rc; }           // the half-built instance frees what it holds
+    I->tipPartAmbig.assign (cfg->tip_count, 0);
     x.tip8 = I->dTip8; x.tip64 = I->dTip64; x.tipPartAmbig = I->dTipPartAmbig; x.partials = I->dPartials; x.matrices = I->dMatrices;
     x.scalers = I->dScalers; x.eigen = I->dEigen; x.weights = I->dWeights; x.invMask = I->dInvMask;
-    x.cijkParts = I->cijkParts; x.patternTiles = 0;
     x.tilePartial = I->dTilePartial; x.tileAbort = I->dTileAbort; x.ticket = I->dTicket;
 
     std::lock_guard<std::mutex> g (gLock);
@@ -1408,7 +1503,7 @@ int mb200_set_pattern_states (int instance, const int *ns, const int *ti, const 
 {
     Instance *I = get (instance);
     if (!I) return MB200_ERROR_BAD_INSTANCE;
-    if (!I->std) return MB200_ERROR_UNSUPPORTED;
+    if (I->family != Family::Std) return MB200_ERROR_UNSUPPORTED;
     const int C = I->cfg.pattern_count, K = I->cfg.category_count;
     if (!ns || !ti || !bs || matLen < 1 || dummy < 0 || dummy > C) return MB200_ERROR_OUT_OF_RANGE;
     int rc = use (I); if (rc) return rc;
@@ -1439,17 +1534,18 @@ int mb200_set_pattern_states (int instance, const int *ns, const int *ti, const 
     CK (cudaMemcpyAsync (dTab + 2*(size_t)C, bs, (size_t)C * sizeof(int), cudaMemcpyHostToDevice, I->stream));
     CK (cudaMemcpyAsync (dClasses, classes.data (), classes.size () * sizeof(int2), cudaMemcpyHostToDevice, I->stream));
     CK (cudaStreamSynchronize (I->stream));
-    I->dStdTab = std::move (dTab); I->dStdClasses = std::move (dClasses); I->dMatrices = std::move (dMats);
+    StdTables &v = I->vs;
+    v.dTab = std::move (dTab); v.dClasses = std::move (dClasses); I->dMatrices = std::move (dMats);
     I->ctx.matrices = I->dMatrices;
     I->ring = MatRing ();                       // its slots hold matrices of the old length
-    I->hNStates.assign (ns, ns + C); I->hTiIndex.assign (ti, ti + C); I->hBsIndex.assign (bs, bs + C);
-    I->hClOff.assign (C + 1, 0);
-    for (int c = 0; c < C; c++) I->hClOff[c + 1] = I->hClOff[c] + (size_t) ns[c];
-    I->sx.nStates = I->dStdTab; I->sx.tiIndex = I->dStdTab + C; I->sx.bsIndex = I->dStdTab + 2*(size_t)C;
-    I->sx.classes = I->dStdClasses; I->sx.nClasses = (int) classes.size ();
-    I->sx.matLen = matLen; I->sx.dummy = dummy; I->sx.uncompressed = uncompressed;
-    I->stdUniformMk = true;
-    I->stdReady = true;
+    v.hNStates.assign (ns, ns + C); v.hTiIndex.assign (ti, ti + C); v.hBsIndex.assign (bs, bs + C);
+    v.hClOff.assign (C + 1, 0);
+    for (int c = 0; c < C; c++) v.hClOff[c + 1] = v.hClOff[c] + (size_t) ns[c];
+    v.sx.nStates = v.dTab; v.sx.tiIndex = v.dTab + C; v.sx.bsIndex = v.dTab + 2*(size_t)C;
+    v.sx.classes = v.dClasses; v.sx.nClasses = (int) classes.size ();
+    v.sx.matLen = matLen; v.sx.dummy = dummy; v.sx.uncompressed = uncompressed;
+    v.uniformMk = true;
+    v.ready = true;
     return MB200_SUCCESS;
 }
 
@@ -1509,7 +1605,7 @@ int mb200_set_rate_matrices (int instance, int eigen, int like_eigen, const doub
     if (!I) return MB200_ERROR_BAD_INSTANCE;
     if (eigen < 0 || eigen >= I->cfg.eigen_count || like_eigen >= I->cfg.eigen_count || !Q || !pi) return MB200_ERROR_OUT_OF_RANGE;
     const int S = I->cfg.state_count, parts = I->cijkParts;
-    if (I->std || S < 2 || S > MB200_EIG_NMAX) return MB200_ERROR_UNSUPPORTED;
+    if (I->family == Family::Std || S < 2 || S > MB200_EIG_NMAX) return MB200_ERROR_UNSUPPORTED;
     for (int s = 0; s < S; s++)
         if (!(pi[s] > 0.0)) return MB200_ERROR_OUT_OF_RANGE;           // sqrt(pi) scales the similarity transform
     int rc = use (I); if (rc) return rc;
@@ -1663,14 +1759,15 @@ int mb200_get_partials (int instance, int buffer, float *out)
     CK (cudaMemcpyAsync (tmp.data (), I->dPartials + (size_t)(buffer - I->cfg.tip_count) * n, n * sizeof(float),
                          cudaMemcpyDeviceToHost, I->stream));
     CK (cudaStreamSynchronize (I->stream));
-    if (I->std)
+    if (I->family == Family::Std)
         {
-        if (!I->stdReady) return MB200_ERROR_UNSUPPORTED;
-        const size_t numReps = I->hClOff[C];                // ragged [k][c][nStates[c]] (src/likelihood.c:1941-1943)
+        const StdTables &v = I->vs;
+        if (!v.ready) return MB200_ERROR_UNSUPPORTED;
+        const size_t numReps = v.hClOff[C];                 // ragged [k][c][nStates[c]] (src/likelihood.c:1941-1943)
         for (int k = 0; k < K; k++)
             for (int c = 0; c < C; c++)
-                for (int s = 0; s < I->hNStates[c]; s++)
-                    out[(size_t)k * numReps + I->hClOff[c] + s] = tmp[((size_t)k * C + c) * Sp + s];
+                for (int s = 0; s < v.hNStates[c]; s++)
+                    out[(size_t)k * numReps + v.hClOff[c] + s] = tmp[((size_t)k * C + c) * Sp + s];
         return MB200_SUCCESS;
         }
     for (size_t r = 0; r < (size_t)K * C; r++)
@@ -1688,14 +1785,15 @@ int mb200_set_partials (int instance, int buffer, const float *in)
     const int S = I->cfg.state_count, K = I->cfg.category_count, C = I->cfg.pattern_count, Sp = I->ctx.Sp;
     const size_t n = (size_t)K * C * Sp;
     std::vector<float> tmp (n, 0.0f);
-    if (I->std)
+    if (I->family == Family::Std)
         {
-        if (!I->stdReady) return MB200_ERROR_UNSUPPORTED;
-        const size_t numReps = I->hClOff[C];
+        const StdTables &v = I->vs;
+        if (!v.ready) return MB200_ERROR_UNSUPPORTED;
+        const size_t numReps = v.hClOff[C];
         for (int k = 0; k < K; k++)
             for (int c = 0; c < C; c++)
-                for (int s = 0; s < I->hNStates[c]; s++)
-                    tmp[((size_t)k * C + c) * Sp + s] = in[(size_t)k * numReps + I->hClOff[c] + s];
+                for (int s = 0; s < v.hNStates[c]; s++)
+                    tmp[((size_t)k * C + c) * Sp + s] = in[(size_t)k * numReps + v.hClOff[c] + s];
         }
     else
     for (size_t r = 0; r < (size_t)K * C; r++)
@@ -1713,8 +1811,9 @@ int mb200_get_transition_matrix (int instance, int matrix, float *out)
     if (!I) return MB200_ERROR_BAD_INSTANCE;
     if (matrix < 0 || matrix >= I->cfg.matrix_count || !out) return MB200_ERROR_OUT_OF_RANGE;
     int rc = use (I); if (rc) return rc;
-    if (I->std && !I->stdReady) return MB200_ERROR_UNSUPPORTED;
-    const size_t n = I->std ? (size_t) I->sx.matLen : (size_t)I->cfg.category_count * I->cfg.state_count * I->cfg.state_count;
+    const bool isStd = (I->family == Family::Std);
+    if (isStd && !I->vs.ready) return MB200_ERROR_UNSUPPORTED;
+    const size_t n = isStd ? (size_t) I->vs.sx.matLen : (size_t)I->cfg.category_count * I->cfg.state_count * I->cfg.state_count;
     CK (cudaMemcpyAsync (out, I->dMatrices + (size_t)matrix * n, n * sizeof(float), cudaMemcpyDeviceToHost, I->stream));
     CK (cudaStreamSynchronize (I->stream));
     return MB200_SUCCESS;
@@ -1726,11 +1825,13 @@ int mb200_set_transition_matrix (int instance, int matrix, const float *in)
     if (!I) return MB200_ERROR_BAD_INSTANCE;
     if (matrix < 0 || matrix >= I->cfg.matrix_count || !in) return MB200_ERROR_OUT_OF_RANGE;
     int rc = use (I); if (rc) return rc;
-    if (I->std && !I->stdReady) return MB200_ERROR_UNSUPPORTED;
-    const size_t n = I->std ? (size_t) I->sx.matLen : (size_t)I->cfg.category_count * I->cfg.state_count * I->cfg.state_count;
-    if (I->std) I->stdUniformMk = false;        // a caller-supplied matrix need not have the Mk form: read every entry from now on
+    const bool isStd = (I->family == Family::Std);
+    if (isStd && !I->vs.ready) return MB200_ERROR_UNSUPPORTED;
+    const size_t n = isStd ? (size_t) I->vs.sx.matLen : (size_t)I->cfg.category_count * I->cfg.state_count * I->cfg.state_count;
+    if (isStd) I->vs.uniformMk = false;        // a caller-supplied matrix need not have the Mk form: read every entry from now on
+    const bool tensor = (I->family == Family::Tensor);
     const int MAT_RING = 64;
-    if (!I->tcS && n * sizeof(float) <= 64*1024)
+    if (!tensor && n * sizeof(float) <= 64*1024)
         {
         // small matrices (host-built P(t) of a STANDARD division, one call per dirty branch): stage through a pinned ring and let
         // the copy ride the instance's stream -- the evaluation that reads the matrix is queued behind it; no host wait
@@ -1750,12 +1851,12 @@ int mb200_set_transition_matrix (int instance, int matrix, const float *in)
         return MB200_SUCCESS;
         }
     CK (cudaMemcpyAsync (I->dMatrices + (size_t)matrix * n, in, n * sizeof(float), cudaMemcpyHostToDevice, I->stream));
-    if (I->tcS)
+    if (tensor)
         {
         const int K = I->cfg.category_count;
-        withTcS (I->tcS, [&] (auto s)
+        withTcS (I->cfg.state_count, [&] (auto s)
             {
-            tc_split_kernel<decltype (s)::value><<<dim3 (1, K), 128, 0, I->stream>>> (I->dMatrices, I->dSplit, nullptr, matrix, K);
+            tc_split_kernel<decltype (s)::value><<<dim3 (1, K), 128, 0, I->stream>>> (I->dMatrices, I->tc.dSplit, nullptr, matrix, K);
             });
         I->launchKind[MB200_KERNEL_SETUP]++;
         }
