@@ -336,6 +336,11 @@ int mb200_get_launch_count (int instance, long long *launches);
 #define MB200_KERNEL_TIPROBS  4
 #define MB200_KERNEL_SETUP    5
 #define MB200_KERNEL_KINDS    6
+/* two sub-counts of the 4-state launches, for the same purpose (not added into mb200_get_launch_count): the job
+ * read from the kernel's parameter block, and throughput mode's one CTA per evaluation (MB200_CONFIG_THROUGHPUT) */
+#define MB200_KERNEL_NUC4_PARAMS    6
+#define MB200_KERNEL_NUC4_PER_EVAL  7
+#define MB200_KERNEL_COUNTERS       8
 int mb200_get_kernel_launches (int instance, int kind, long long *launches);
 /* Device-side timing of the dominant (fused pruning) kernel: when enabled, every launch of
  * it is bracketed by CUDA events on the instance's stream.  mb200_get_kernel_time

@@ -25,6 +25,7 @@ NONE = -1
 CONFIG_THROUGHPUT = 1        # mb200_instance_config.flags: favour throughput over single-call latency
 CONFIG_VARIABLE_STATES = 2   # STANDARD-data division: per-pattern state counts (the *_Std kernel family)
 KERNEL_NUC4, KERNEL_TENSOR, KERNEL_GENERIC, KERNEL_STD, KERNEL_TIPROBS, KERNEL_SETUP = range(6)
+KERNEL_NUC4_PARAMS, KERNEL_NUC4_PER_EVAL = 6, 7      # 4-state sub-counts (include/mb200.h)
 EIGEN_INLINE = -2
 FLAG_NUC4_PINVAR_QUIRK = 1
 FLAG_TIP_SHORTCUTS = 2

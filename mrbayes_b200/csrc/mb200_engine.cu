@@ -212,6 +212,7 @@ struct Instance
     int           cijkParts = 1;       // eigensystems per slot (one per category for NY98-type models)
     size_t        smemGen = 0;         // generic family: dynamic smem of eval_gen_kernel
     long long     launchKind[MB200_KERNEL_KINDS] = {0};   // per kernel family (mb200_get_kernel_launches)
+    long long     launchNuc4Sub[MB200_KERNEL_COUNTERS - MB200_KERNEL_KINDS] = {0};   // 4-state sub-counts (same)
     std::vector<int> tipPartAmbig;  // host copy (operand kinds of the 4-state records)
     int           tipEpoch = 0;
     int           writtenStamp = 0;
@@ -801,7 +802,10 @@ int launchNuc4 (Instance *I, const Batch &b, DevCtx &ctx, bool viaParams, bool t
     // the latency of one launch -- one CTA per evaluation walks all its tiles and builds P(t) once
     // instead of once per tile.  Single-chunk evaluations only (per-pattern state lives in registers).
     if (b.fused && (I->cfg.flags & MB200_CONFIG_THROUGHPUT) && b.singleChunk)
+        {
         ctx.numTiles = 1;
+        I->launchNuc4Sub[MB200_KERNEL_NUC4_PER_EVAL - MB200_KERNEL_KINDS]++;
+        }
     ctx.hostSum = (toHost && b.allRoot && b.fused && ctx.numTiles <= HOSTSUM_MAX_TILES) ? 1 : 0;
     const dim3 grid (ctx.numTiles, b.nEval);
     const BlobOffsets off = { (int) b.offEval, (int) b.offDbl, (int) b.offUpd, (int) b.offChunk, (int) b.offCmat, (int) b.offOp };
@@ -834,6 +838,8 @@ int launchNuc4 (Instance *I, const Batch &b, DevCtx &ctx, bool viaParams, bool t
         });
     if (rc != MB200_SUCCESS) return rc;
     I->launchKind[MB200_KERNEL_NUC4]++;
+    if (viaParams)
+        I->launchNuc4Sub[MB200_KERNEL_NUC4_PARAMS - MB200_KERNEL_KINDS]++;
     return MB200_SUCCESS;
 }
 
@@ -2007,8 +2013,8 @@ int mb200_get_kernel_launches (int instance, int kind, long long *launches)
 {
     Instance *I = get (instance);
     if (!I || !launches) return MB200_ERROR_BAD_INSTANCE;
-    if (kind < 0 || kind >= MB200_KERNEL_KINDS) return MB200_ERROR_OUT_OF_RANGE;
-    *launches = I->launchKind[kind];
+    if (kind < 0 || kind >= MB200_KERNEL_COUNTERS) return MB200_ERROR_OUT_OF_RANGE;
+    *launches = (kind < MB200_KERNEL_KINDS) ? I->launchKind[kind] : I->launchNuc4Sub[kind - MB200_KERNEL_KINDS];
     return MB200_SUCCESS;
 }
 

@@ -38,13 +38,80 @@ def tip_partials(pr, tip):
     return bits.astype(np.float64)
 
 
-def f64_lnl(pr, ch, tree=None, *, Q=None, freqs=None, rates=None, cat_weights=None, p_invar=None, weights=None):
-    """-> (per-pattern log likelihoods [C], lnL) of chain `ch` on its current tree.
+# ---- the root with an invariable-sites category ------------------------------------------------------------------
+# A pattern's likelihood is (1 - p) L + p L_I, with L = exp(lnScaler) like the rescaled root sum.  MrBayes cannot
+# exponentiate a site scaler below SCALER_SWITCH, so there it approximates, and two of its likelihood families do so
+# differently.  Three rules, per pattern, with s the site scaler the decision reads:
+#   ROOT_EXACT  logaddexp(lnScaler + log like, log likeI), the mixture itself;
+#   ROOT_GEN    Likelihood_Gen / _Gen_SSE: s >= -200: log(like + likeI / exp(lnScaler)) + lnScaler;
+#               s < -200: log likeI if likeI > LIKE_I_MIN (like is negligible beside it), else lnScaler + log like
+#               (likeI is dropped, even where it dominates);
+#   ROOT_QUIRK  Likelihood_NUC4_* (MB200_FLAG_NUC4_PINVAR_QUIRK): as ROOT_GEN, except that for s < -200 and
+#               likeI > LIKE_I_MIN the term is lnScaler + log likeI -- the scaler is added to a likelihood that was
+#               never scaled.
+# ROOT_GEN equals ROOT_EXACT except where s < -200 and 0 < likeI <= LIKE_I_MIN (it is lower there); ROOT_QUIRK equals
+# ROOT_GEN except where s < -200 and likeI > LIKE_I_MIN (lower by |lnScaler|).
+ROOT_EXACT, ROOT_GEN, ROOT_QUIRK = "exact", "gen", "quirk"
+SCALER_SWITCH = -200.0
+LIKE_I_MIN = 1e-70
+FLAG_NUC4_PINVAR_QUIRK = 1                    # MB200_FLAG_NUC4_PINVAR_QUIRK (include/mb200.h)
+# which side of the switch a pattern is on (RootTerms.branch)
+ABOVE_SWITCH, INVAR_DOMINATES, INVAR_TINY, INVAR_ZERO = 0, 1, 2, 3
+
+
+class RootTerms:
+    """f64_root's result: per-pattern log likelihoods (site) and lnL; the float64 site scalers (lnscale), the rescaled
+    root sums (like) and the invariable-site likelihoods p L_I (like_i); with p_invar, per pattern which branch of the
+    rule it took (branch: ABOVE_SWITCH, or below the switch INVAR_DOMINATES (likeI > LIKE_I_MIN), INVAR_TINY
+    (0 < likeI <= LIKE_I_MIN) or INVAR_ZERO), else None"""
+
+    def __init__(self, site, lnl, lnscale, like, like_i, branch):
+        self.site, self.lnl, self.lnscale, self.like, self.like_i, self.branch = site, lnl, lnscale, like, like_i, branch
+
+
+def root_rule_of(flags):
+    """the rule an evaluation with these flags asks for: ROOT_QUIRK with MB200_FLAG_NUC4_PINVAR_QUIRK, else ROOT_GEN"""
+    return ROOT_QUIRK if int(flags) & FLAG_NUC4_PINVAR_QUIRK else ROOT_GEN
+
+
+def root_site_terms(lnscale, like, like_i, rule, scalers=None):
+    """-> (per-pattern log likelihoods, branch) under `rule`.  The terms use the float64 lnscale; the decision at
+    SCALER_SWITCH reads `scalers` if given (a float site-scaler vector read back from an engine or the oracle, so
+    that a pattern near -200 branches as it did there), else lnscale."""
+    s = np.asarray(lnscale if scalers is None else scalers, np.float64)
+    below_switch = s < SCALER_SWITCH
+    branch = np.where(~below_switch, ABOVE_SWITCH,
+                      np.where(like_i > LIKE_I_MIN, INVAR_DOMINATES, np.where(like_i > 0, INVAR_TINY, INVAR_ZERO)))
+    with np.errstate(divide="ignore", over="ignore"):
+        log_like_i = np.log(like_i)
+        exact = np.logaddexp(lnscale + np.log(like), log_like_i)
+        if rule == ROOT_EXACT:
+            return exact, branch
+        mixed = lnscale + np.log(like + like_i * np.exp(np.minimum(-lnscale, 700.0)))
+        dominated = log_like_i + (lnscale if rule == ROOT_QUIRK else 0.0)
+    assert rule in (ROOT_GEN, ROOT_QUIRK), rule
+    site = np.where(branch == ABOVE_SWITCH, mixed,
+                    np.where(branch == INVAR_DOMINATES, dominated, lnscale + np.log(like)))
+    return site, branch
+
+
+def f64_lnl(pr, ch, tree=None, **kw):
+    """-> (per-pattern log likelihoods [C], lnL) of chain `ch` on its current tree: f64_root's"""
+    r = f64_root(pr, ch, tree, **kw)
+    return r.site, r.lnl
+
+
+def f64_root(pr, ch, tree=None, *, Q=None, freqs=None, rates=None, cat_weights=None, p_invar=None, weights=None,
+             flags=None, rule=None, scalers=None, pmat_cache=None):
+    """Float64 pruning of chain `ch` on its current tree -> RootTerms.
 
     Without overrides the model is the problem's: its eigensystem, frequencies, rates / (1 - p_invar) and
     equal category weights (1 - p_invar) / K.  Overrides describe one evaluation's own model: Q (per-category
     rate matrices, see transition_matrices), freqs, rates and cat_weights exactly as the evaluation sends
-    them, p_invar (0: none) and the pattern weights of its weights row."""
+    them, p_invar (0: none) and the pattern weights of its weights row.  With p_invar the root follows `rule`
+    (ROOT_EXACT, ROOT_GEN or ROOT_QUIRK; default the one `flags` ask for, default the problem's flags), its
+    decision at the switch read from `scalers` if given (root_site_terms).  pmat_cache, a dict the caller keeps
+    across calls with the same model, holds P(t) by branch length, for long runs of branch updates."""
     tr = pr.tree[ch] if tree is None else tree
     pinv = pr.p_invar if p_invar is None else float(p_invar)
     freqs = np.asarray(pr.freqs if freqs is None else freqs, float)
@@ -54,7 +121,12 @@ def f64_lnl(pr, ch, tree=None, *, Q=None, freqs=None, rates=None, cat_weights=No
     cl, lnscale = {}, np.zeros(pr.C)
 
     def pmat(node):
-        return transition_matrices(pr, tr.length[node], rates, Q, freqs)
+        t = float(tr.length[node])
+        if pmat_cache is None:
+            return transition_matrices(pr, t, rates, Q, freqs)
+        if t not in pmat_cache:
+            pmat_cache[t] = transition_matrices(pr, t, rates, Q, freqs)
+        return pmat_cache[t]
 
     def child(node):
         x = np.broadcast_to(tip_partials(pr, node), (pr.K, pr.C, pr.S)) if node < tr.n_tips else cl[node]
@@ -65,22 +137,78 @@ def f64_lnl(pr, ch, tree=None, *, Q=None, freqs=None, rates=None, cat_weights=No
         if tr.anc[p] == tr.root:                       # the interior root also takes the root tip
             rt = tip_partials(pr, tr.root)[None]
             x = x * np.einsum("kij,kcj->kci", pmat(p), np.broadcast_to(rt, x.shape))
+            # ...and is not rescaled, as in MrBayes: the site scaler holds the other nodes' scalers only, which
+            # matters where a root rule adds it to a likelihood it did not scale (ROOT_QUIRK)
+            cl[p] = x
+            continue
         m = x.max(axis=(0, 2))
         m = np.where(m > 0, m, 1.0)
         cl[p] = x / m[None, :, None]
         lnscale += np.log(m)
     like = np.einsum("k,kcs,s->c", catw, cl[tr.root_left], freqs)
+    like_i, branch = np.zeros(pr.C), None
     if pinv > 0:
         inv = np.bitwise_and.reduce(pr.masks, axis=0)
         bits = (inv[:, None] >> np.arange(pr.S, dtype=np.uint64)[None, :]) & np.uint64(1)
-        like_i = pinv * (bits * freqs[None, :]).sum(1)
-        # Likelihood_Gen's formula; below a scaler of -200 the reference switches to an approximation
-        assert lnscale.min() >= -200.0, "site scaler below -200: the reference approximates there"
-        site = lnscale + np.log(like + like_i * np.exp(-lnscale))
+        # the 4-state family takes p_invar as a float (Likelihood_NUC4_*: (CLFlt) pInvar), so below FLT_TRUE_MIN it
+        # is 0 and likeI with it: 0 < likeI <= LIKE_I_MIN (INVAR_TINY) cannot occur on 4 states
+        p = float(np.float32(pinv)) if pr.S == 4 else pinv
+        like_i = p * (bits * freqs[None, :]).sum(1)
+        rule = root_rule_of(pr.flags if flags is None else flags) if rule is None else rule
+        site, branch = root_site_terms(lnscale, like, like_i, rule, scalers)
     else:
         with np.errstate(divide="ignore"):
             site = lnscale + np.log(like)
-    return site, float(site @ weights)
+    return RootTerms(site, float(site @ weights), lnscale, like, like_i, branch)
+
+
+# ---- how far float site scalers may drift from float64 ------------------------------------------------------------
+# An engine (and MrBayes) keeps a pattern's site scaler as a float sum: a full evaluation resets it and adds one node
+# scaler per rescaled node, each branch update removes the replaced nodes' scalers and adds the new ones, a rejected
+# update flips back to the previous vector.  Each addition or removal rounds to the nearest float, an error of at most
+# half an ulp of the value it lands on; each node scaler is itself log(max) rounded to float, half an ulp of the node
+# scaler.  Node scalers are logs of maxima <= 1, so all of them are <= 0: a node scaler is no larger than the site
+# scaler it is part of, and every partial sum on the way from a vector s_src to its update s_dst is bounded by
+# |s_src| + |s_dst| (removals move towards 0; the additions are a subset of s_dst's terms).  With M_c the largest
+# such bound since the last reset, n the additions and removals since then and m the node scalers in the sum, the
+# site scaler of pattern c is off by at most (n + m) ulp(M_c) / 2, and lnL, which adds each site scaler w_c times, by
+#     drift = sum_c w_c (n + m) ulp(M_c) / 2.
+# At a thousand tips this is far above a few float ulps of lnL: a 4-state full evaluation at 1000 tips rounds ~1000
+# times into values of a few hundred.  The bar a float evaluation meets against float64 is the small-tree relative
+# bar for everything else (P(t), partials, the root sum) plus this drift.
+def half_ulp(x):
+    """half the float32 ulp of |x|, elementwise, in double"""
+    return np.spacing(np.abs(np.asarray(x, np.float64)).astype(np.float32)).astype(np.float64) / 2
+
+
+class ScalerLedger:
+    """Per site-scaler buffer: the additions and removals (n) and node scalers (m) its float sum has taken since its
+    last reset, and M_c of every pattern -- the drift bound above.  record() each evaluation with the site scalers it
+    wrote (read back, float); a rejection needs nothing, since the restored buffer's entry is still here."""
+
+    def __init__(self):
+        self.book = {}                                   # site buffer -> (n, m, M [C], s [C])
+
+    def record(self, sp, site_scalers):
+        s = np.abs(np.asarray(site_scalers, np.float64))
+        writes = int((sp.ops["scale_write"] >= 0).sum())
+        removes = int((sp.ops["scale_remove"] >= 0).sum())
+        if sp.site_src < 0:
+            n, m, M = writes, writes, s
+        else:
+            n0, m, M0, s0 = self.book[int(sp.site_src)]
+            n, M = n0 + writes + removes, np.maximum(M0, s0 + s)
+            m += writes - removes
+        self.book[int(sp.site_dst)] = (n, m, M, s)
+
+    def pattern_bound(self, sp):
+        """[C] how far each float site scaler of sp's destination may be from float64: (n + m) ulp(M_c) / 2"""
+        n, m, M, _ = self.book[int(sp.site_dst)]
+        return (n + m) * half_ulp(M)
+
+    def drift(self, sp, weights):
+        """the bound on |lnL - lnL64| the float site scalers of sp's destination may carry"""
+        return float(np.asarray(weights, np.float64) @ self.pattern_bound(sp))
 
 
 # ----------------------------------------------------------------------------- variable-state (Std) divisions

@@ -5,7 +5,7 @@ only judge of the engine there, is itself checked; and the tree builders the GPU
 import numpy as np
 import pytest
 
-from f64_reference import balanced_tree, caterpillar_tree, f64_lnl, transition_matrices, tree_height
+from f64_reference import balanced_tree, caterpillar_tree, f64_lnl, f64_root, transition_matrices, tree_height
 from mrbayes_b200 import abi, workloads
 
 # float oracle vs double reference: float rounding in P(t), in the node products and in the scalers
@@ -287,3 +287,104 @@ def test_f64_std_reference_matches_cynmix_golden():
         ref = f64_std_lnl(pr, sp.chain, tree_from_evaluation(sp, n_tips), rates=sp.rates)
         assert not ref.underflow and 0.0 < ref.p_un < 1.0
         assert abs(ref.lnl - sp.lnl_ref) < RTOL * abs(sp.lnl_ref), f"chain {sp.chain}: {ref.lnl!r} vs {sp.lnl_ref!r}"
+
+
+# ---- the root with invariable sites past the -200 site-scaler switch, at a few hundred to a thousand tips -------------
+SWITCH_CASES = [
+    # S, K, C, tips, mean branch length
+    (4, 1, 256, 1000, 0.15),
+    (4, 4, 256, 600, 0.25),
+    (20, 1, 64, 300, 0.4),
+    (20, 4, 64, 400, 0.4),
+    (61, 1, 32, 300, 0.5),
+    (61, 4, 32, 300, 0.5),
+]
+
+
+@pytest.mark.parametrize("S,K,C,tips,mean", SWITCH_CASES)
+def test_root_rules_past_scaler_switch(oracle_lib, S, K, C, tips, mean):
+    """Each chain evaluates under one of root_variants (quirk flag on or off, p_invar 0.2 or 1e-80).  The oracle's lnL
+    is the float64 reference's under the rule its flags ask for, the decision at -200 read from the oracle's site
+    scalers, within the small-tree bar plus the scaler drift.  The quirk moves lnL by thousands of log units and ROOT_GEN
+    is ROOT_EXACT except where it drops a tiny likeI.  Every branch of the rule occurs, except INVAR_TINY on 4 states,
+    where p_invar is a float and 1e-80 is 0."""
+    from engine_checks import root_variants, switch_problem, variant_root, with_root_variant
+    from f64_reference import (ABOVE_SWITCH, INVAR_DOMINATES, INVAR_TINY, INVAR_ZERO, ROOT_EXACT, ROOT_GEN, ROOT_QUIRK,
+                               ScalerLedger, root_site_terms)
+    pr = switch_problem(S, K, C, tips, 4, seed=10 + S + K, mean_len=mean)
+    pr.tree[1] = caterpillar_tree(tips, np.random.default_rng(S), mean_len=mean)
+    pr.tree[2] = balanced_tree(tips, np.random.default_rng(K), mean_len=mean)
+    seen = set()
+    with pr.create(oracle_lib) as o:
+        o.set_arith(1)
+        for ch in range(4):
+            sp = with_root_variant(pr, pr.full_evaluation(ch))
+            (lo,), (so,) = o.evaluate(sp)
+            assert so == abi.EVAL_OK
+            sc = o.get_scalers(sp.site_dst)
+            ledger = ScalerLedger()
+            ledger.record(sp, sc)
+            ref = variant_root(pr, sp, sc)
+            bar = RTOL * abs(ref.lnl) + ledger.drift(sp, pr.weights)
+            assert abs(lo - ref.lnl) <= bar, f"chain {ch}: oracle {lo!r}, float64 {ref.lnl!r}, bar {bar:.2e}"
+            seen |= set(ref.branch.tolist())
+            # the other rules on the same terms, and where they part
+            args = (ref.lnscale, ref.like, ref.like_i)
+            exact, _ = root_site_terms(*args, ROOT_EXACT, sc)
+            gen, _ = root_site_terms(*args, ROOT_GEN, sc)
+            quirk, _ = root_site_terms(*args, ROOT_QUIRK, sc)
+            tiny = ref.branch == INVAR_TINY
+            assert np.allclose(gen[~tiny], exact[~tiny], rtol=1e-12, atol=1e-12)
+            assert (gen[tiny] < exact[tiny] - 1.0).all()                        # the dropped likeI dominated
+            dom = ref.branch == INVAR_DOMINATES
+            assert np.array_equal(quirk[~dom], gen[~dom])
+            assert np.allclose(quirk[dom], gen[dom] + ref.lnscale[dom], rtol=1e-12)
+            if dom.any():
+                assert abs(float((quirk - gen) @ pr.weights)) > 1e3
+            flags, _ = root_variants(pr)[ch]
+            assert np.array_equal(ref.site, quirk if flags & abi.FLAG_NUC4_PINVAR_QUIRK else gen)
+    want = {ABOVE_SWITCH, INVAR_DOMINATES, INVAR_ZERO} | ({INVAR_TINY} if S != 4 else set())
+    assert seen == want, seen
+
+
+@pytest.mark.parametrize("S,K,C,tips,updates", [(4, 4, 256, 1000, 60), (61, 2, 32, 300, 60)])
+def test_scaler_drift_bar_long_run(oracle_lib, S, K, C, tips, updates):
+    """A full evaluation per chain (a random tree and a caterpillar), then branch updates with every third rejected: the
+    oracle stays within the small-tree bar plus the site-scaler drift (f64_reference.ScalerLedger) of float64 at every
+    step, and each chain's drift term grows with its updates.  At the end a fresh full evaluation of each chain's tree
+    shows the drift itself: the updated float site scalers differ from the fresh ones, and by no more than the two
+    vectors' per-pattern bounds."""
+    from engine_checks import evaluation_sequence
+    from f64_reference import ScalerLedger
+    pr = workloads.make_problem(S, K, C, tips, 2, seed=20 + S, p_ambig=0.05)
+    pr.tree[1] = caterpillar_tree(tips, np.random.default_rng(S))
+    ledger = ScalerLedger()
+    drifts = {0: [], 1: []}
+    last = {}
+    cache = {}
+    with pr.create(oracle_lib) as o:
+        o.set_arith(1)
+        for it, sp in evaluation_sequence(pr, updates, seed=S):
+            (lo,), (so,) = o.evaluate(sp)
+            assert so == abi.EVAL_OK
+            ledger.record(sp, o.get_scalers(sp.site_dst))
+            lf = f64_root(pr, sp.chain, pmat_cache=cache).lnl
+            drift = ledger.drift(sp, pr.weights)
+            drifts[sp.chain].append(drift)
+            assert abs(lo - lf) <= RTOL * abs(lf) + drift, f"evaluation {it}: {lo!r} vs {lf!r}, drift {drift:.2e}"
+            if it % 3 != 2:                               # the state the chain keeps
+                last[sp.chain] = sp
+        assert all(d[-1] > d[0] for d in drifts.values())
+        for ch in range(2):
+            # the last kept update's site scalers against a fresh full evaluation of the same tree
+            kept = last[ch] if last[ch].site_dst == pr.chains[ch].site else None
+            assert kept is not None
+            updated = o.get_scalers(kept.site_dst).astype(np.float64)
+            bound = ledger.pattern_bound(kept)
+            fresh_sp = pr.full_evaluation(ch)
+            o.evaluate(fresh_sp)
+            fresh = o.get_scalers(fresh_sp.site_dst).astype(np.float64)
+            ledger.record(fresh_sp, fresh)
+            d = np.abs(updated - fresh)
+            assert d.max() > 0.0, f"chain {ch}"
+            assert (d <= bound + ledger.pattern_bound(fresh_sp)).all(), f"chain {ch}: {d.max():.2e}"
