@@ -260,15 +260,25 @@ int mb200_set_eigen_decomposition (int instance, int eigen, const double *eigvec
 int mb200_set_rate_matrices (int instance, int eigen, int like_eigen, const double *rate_matrices, const double *state_freqs);
 
 /* ---- node-granular verbs (the function-pointer / BEAGLE-verb level) ---------------- */
+/* category_rates[category_count]; state_freqs[state_count]: the stationary rows of branches with
+ * r t > TIME_MAX.  state_freqs may be NULL on variable-state instances only (their Mk matrices do
+ * not read it); elsewhere NULL is MB200_ERROR_OUT_OF_RANGE, whatever count is.  Updates whose
+ * eigen is MB200_EIGEN_INLINE are MB200_ERROR_UNSUPPORTED here (no evaluation carries the
+ * eigensystem). */
 int mb200_update_transition_matrices (int instance, const mb200_matrix_update *updates,
                                       int count, const double *category_rates,
                                       const double *state_freqs);
 /* site_scaler = cumulative scale buffer that node scalers are removed from / added to
- * (MB200_NONE: leave site scalers alone) */
+ * (MB200_NONE: leave site scalers alone).  The call carries no evaluation flags: it never takes
+ * MB200_FLAG_TIP_SHORTCUTS, so a missing observation on a tip contributes the sum of its P(t) row,
+ * as mb200_evaluate computes it without that flag. */
 int mb200_update_partials (int instance, const mb200_operation *operations, int count,
                            int site_scaler);
 int mb200_reset_scalers   (int instance, int scaler);                 /* ResetSiteScalers */
 int mb200_copy_scalers    (int instance, int dst, int src);           /* CopySiteScalers  */
+/* state_freqs as in mb200_evaluation: state_count entries, or on variable-state instances the
+ * whole table the patterns index, max_c (freq_offsets[c] + state_counts[c]) entries (which may
+ * exceed state_count).  category_weights[category_count]. */
 int mb200_root_log_likelihood (int instance, int root_buffer, int site_scaler,
                                int weights_row, const double *state_freqs,
                                const double *category_weights, int has_p_invar,

@@ -124,9 +124,9 @@ class Library:
             "set_partials": [I, I, P(C.c_float)],
             "get_transition_matrix": [I, I, P(C.c_float)],
             "get_scalers": [I, I, P(C.c_float)],
-            # engine only
             "set_transition_matrix": [I, I, P(C.c_float)],
             "set_scalers": [I, I, P(C.c_float)],
+            # engine only
             "update_transition_matrices": [I, P(MatrixUpdate), I, P(D), P(D)],
             "update_partials": [I, P(Operation), I, I],
             "reset_scalers": [I, I],
@@ -404,11 +404,14 @@ class Instance:
         return ms.value, n.value
 
     # -- node-granular verbs --------------------------------------------------------------
-    def update_transition_matrices(self, mats, rates, freqs=None):
+    def update_transition_matrices(self, mats, rates, freqs):
+        """P(t) of the branches in mats; freqs are the stationary rows of branches past TIME_MAX.  None sends NULL,
+        which only variable-state instances accept."""
         mats = np.ascontiguousarray(mats, MAT_DTYPE)
         rates = np.ascontiguousarray(rates, np.float64)
-        f = np.ascontiguousarray(freqs if freqs is not None else np.zeros(self.S), np.float64)
-        self._call("update_transition_matrices", _ptr(mats, MatrixUpdate), len(mats), _ptr(rates, C.c_double), _ptr(f, C.c_double))
+        f = None if freqs is None else np.ascontiguousarray(freqs, np.float64)
+        self._call("update_transition_matrices", _ptr(mats, MatrixUpdate), len(mats), _ptr(rates, C.c_double),
+                   None if f is None else _ptr(f, C.c_double))
 
     def update_partials(self, ops, site_scaler=NONE):
         ops = np.ascontiguousarray(ops, OP_DTYPE)
@@ -447,9 +450,19 @@ class Instance:
         self._call("set_transition_matrix", matrix, _ptr(b, C.c_float))
 
     def set_partials(self, buffer: int, a):
+        """[K, C, S] floats, or for variable-state divisions the ragged layout get_partials returns"""
         a = np.ascontiguousarray(a, np.float32)
-        assert a.shape == (self.K, self.C, self.S)
+        if self.variable_states:
+            assert a.shape == (self.K, int(self.state_counts.sum()))
+        else:
+            assert a.shape == (self.K, self.C, self.S)
         self._call("set_partials", buffer, _ptr(a, C.c_float))
+
+    def set_scalers(self, scaler: int, v):
+        """a node or site scaler buffer: [C] floats"""
+        v = np.ascontiguousarray(v, np.float32)
+        assert v.shape == (self.C,)
+        self._call("set_scalers", scaler, _ptr(v, C.c_float))
 
     def get_transition_matrix(self, matrix: int) -> np.ndarray:
         if self.variable_states:

@@ -186,6 +186,7 @@ struct StdTables                       // variable-state family: mb200_set_patte
     DevArray<int2> dClasses;
     std::vector<int> hNStates, hTiIndex, hBsIndex;
     std::vector<size_t> hClOff;        // ragged host layout: offset of pattern c inside a category's block
+    int           freqLen = 0;         // entries of the frequency table the patterns index: max_c (bsIndex[c] + nStates[c])
 };
 
 struct Instance
@@ -1546,7 +1547,12 @@ int mb200_set_pattern_states (int instance, const int *ns, const int *ti, const 
     I->ring = MatRing ();                       // its slots hold matrices of the old length
     v.hNStates.assign (ns, ns + C); v.hTiIndex.assign (ti, ti + C); v.hBsIndex.assign (bs, bs + C);
     v.hClOff.assign (C + 1, 0);
-    for (int c = 0; c < C; c++) v.hClOff[c + 1] = v.hClOff[c] + (size_t) ns[c];
+    v.freqLen = 0;
+    for (int c = 0; c < C; c++)
+        {
+        v.hClOff[c + 1] = v.hClOff[c] + (size_t) ns[c];
+        if (bs[c] + ns[c] > v.freqLen) v.freqLen = bs[c] + ns[c];
+        }
     v.sx.nStates = v.dTab; v.sx.tiIndex = v.dTab + C; v.sx.bsIndex = v.dTab + 2*(size_t)C;
     v.sx.classes = v.dClasses; v.sx.nClasses = (int) classes.size ();
     v.sx.matLen = matLen; v.sx.dummy = dummy; v.sx.uncompressed = uncompressed;
@@ -1652,7 +1658,10 @@ int mb200_update_transition_matrices (int instance, const mb200_matrix_update *u
 {
     Instance *I = get (instance);
     if (!I) return MB200_ERROR_BAD_INSTANCE;
-    if (count < 0 || (count > 0 && !updates) || !category_rates) return MB200_ERROR_OUT_OF_RANGE;
+    // stationary rows (t > TIME_MAX) are the frequencies: only the variable-state family, whose Mk matrices do not
+    // read them, may leave them out
+    if (count < 0 || (count > 0 && !updates) || !category_rates || (!state_freqs && I->family != Family::Std))
+        return MB200_ERROR_OUT_OF_RANGE;
     if (count == 0) return MB200_SUCCESS;
     int rc = use (I); if (rc) return rc;
     mb200_evaluation ev;
@@ -1718,7 +1727,10 @@ int mb200_root_log_likelihood (int instance, int root_buffer, int site_scaler, i
     ev.site_scaler_dst = MB200_NONE; ev.site_scaler_src = site_scaler; ev.root_buffer = root_buffer;
     ev.weights_row = weights_row; ev.flags = flags; ev.has_p_invar = has_p_invar; ev.p_invar = p_invar;
     for (int k = 0; k < I->cfg.category_count; k++) ev.category_weights[k] = category_weights[k];
-    for (int s = 0; s < I->cfg.state_count; s++) ev.state_freqs[s] = state_freqs[s];
+    // variable-state divisions: the whole table the patterns index (freq_offsets[c] + state_counts[c]), which may
+    // be longer than state_count
+    const int nFreq = (I->family == Family::Std) ? I->vs.freqLen : I->cfg.state_count;
+    for (int s = 0; s < nFreq; s++) ev.state_freqs[s] = state_freqs[s];
     int st = 0;
     rc = runSync (I, &ev, 1, lnL, &st);
     if (status) *status = st;

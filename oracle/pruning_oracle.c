@@ -765,6 +765,16 @@ int orc_get_scalers (int instance, int scaler, float *out)
     return MB200_SUCCESS;
 }
 
+/* a node or site scaler buffer filled by the caller */
+int orc_set_scalers (int instance, int scaler, const float *in)
+{
+    OrcInst *o = Get (instance);
+    if (!o) return MB200_ERROR_BAD_INSTANCE;
+    if (scaler < 0 || scaler >= o->cfg.scaler_count || !in) return MB200_ERROR_OUT_OF_RANGE;
+    memcpy (o->scalers + (size_t)scaler * o->cfg.pattern_count, in, (size_t)o->cfg.pattern_count * sizeof(float));
+    return MB200_SUCCESS;
+}
+
 /* CompressData's uniqueness scan (src/model.c:2618-2686): a column joins the FIRST earlier
  * column that is identical over all taxa, otherwise it becomes a new pattern; weights are
  * integer site counts (tempSitesOfPat). */

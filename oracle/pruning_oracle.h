@@ -39,7 +39,9 @@ int orc_evaluate (int instance, const mb200_evaluation *evaluations, int count,
 int orc_get_partials          (int instance, int buffer, float *out);
 int orc_set_partials          (int instance, int buffer, const float *in);
 int orc_get_transition_matrix (int instance, int matrix, float *out);
+int orc_set_transition_matrix (int instance, int matrix, const float *in);
 int orc_get_scalers           (int instance, int scaler, float *out);
+int orc_set_scalers           (int instance, int scaler, const float *in);
 long long orc_cl_updates      (int instance);   /* node*pattern*rate updates done so far */
 
 /* Site-pattern compression (CompressData, src/model.c:2466-2782), integer, bit-exact:

@@ -445,3 +445,170 @@ def eigen_instance(lib, S, K, parts):
     flags = (parts << 8) if parts > 1 else 0
     return abi.Instance(lib, tip_count=2, partials_count=4, state_count=S, pattern_count=16, category_count=K,
                         matrix_count=6, scaler_count=2, eigen_count=3, flags=flags)
+
+
+# ---- one call against the float64 reference over the buffers it read (f64_reference.f64_evaluation) ---------------
+ULP = 2.0 ** -23                                 # float ulp of 1
+
+
+def f64_inputs(inst, sp):
+    """-> (partials, matrices, scalers) sp reads, read back from inst (engine or oracle) now: its interior operands and
+    root buffer, the matrices of its operations and the scalers it removes and copies"""
+    tips = inst.cfg.tip_count
+    parts, mats, scal = {}, {}, {}
+    for op in sp.ops:
+        for c, m in ((op["child1"], op["matrix1"]), (op["child2"], op["matrix2"]), (op["child3"], op["matrix3"])):
+            if c < 0:
+                continue
+            if c >= tips and int(c) not in parts:
+                parts[int(c)] = inst.get_partials(int(c))
+            mats.setdefault(int(m), inst.get_transition_matrix(int(m)))
+        if op["scale_remove"] >= 0:
+            scal[int(op["scale_remove"])] = inst.get_scalers(int(op["scale_remove"]))
+    if sp.site_src >= 0:
+        scal[sp.site_src] = inst.get_scalers(sp.site_src)
+    if sp.root >= 0:
+        parts.setdefault(sp.root, inst.get_partials(sp.root))
+    return parts, mats, scal
+
+
+def f64_call_check(inst, pr, sp, ref, tensor, status=None, lnl=None):
+    """Every buffer sp wrote on inst, and its lnL, against ref = f64_evaluation of the same call on the same inputs.
+
+    Off the tensor cores every term is non-negative, so a node carries at most about S + 3 roundings (the S-term dot
+    product, the products of its children, the division by its peak) on top of its children's error: the partials bar
+    is (S + 3) float ulps relative per operation of the call in the node's subtree (Evaluation64.below), with an absolute
+    floor of as many flushed subnormal results (FLT_MIN each) divided by the node's peak.  On the tensor cores
+    subtree_tol's per-node term counted within the call, 2e-5 + 1e-6 per operation below, with a floor of three flushed
+    products per term (the 3xTF32 split) of each operation below, divided by the peak.  A node scaler is the log of the peak: the node's bar before rescaling plus half a float
+    ulp of the scaler; a site scaler adds its node scalers' bars and half an ulp of its running size per addition and
+    removal.  lnL: lnl_tol(S) relative (plus, for Std, the coding-bias conditioning).  -> the largest fraction of a bar
+    used."""
+    from f64_reference import half_ulp
+    S = pr.S
+    used = 0.0
+    node_bar = {}
+    for op in sp.ops:
+        dest = int(op["dest"])
+        n = ref.below[dest]
+        want = ref.partials[dest]
+        got = inst.get_partials(dest).astype(np.float64)
+        # the floor: a product below FLT_MIN may be flushed to zero (the tensor cores flush subnormals, and so may the
+        # other kernels), an error below FLT_MIN per product -- three per term with the 3xTF32 split -- which the
+        # division by the node's peak enlarges
+        if tensor:
+            rtol, floor = 2e-5 + 1e-6 * n, n * 3 * S * FLT_MIN / ref.peak[dest]
+        else:
+            rtol, floor = n * (S + 3) * ULP, n * (S + 3) * FLT_MIN / ref.peak[dest]
+        atol = floor[None, :, None] if want.ndim == 3 else np.repeat(floor, pr.state_counts)[None, :]
+        bar = atol + rtol * np.abs(want)
+        frac = np.abs(got - want) / bar
+        worst = float(frac.max())
+        assert worst <= 1.0, f"partials of buffer {dest}: {worst:.2f} x the float64 bar (rtol {rtol:.2e}, {n} below)"
+        used = max(used, worst)
+        if op["scale_write"] >= 0:
+            w = int(op["scale_write"])
+            node_bar[w] = rtol + half_ulp(ref.scalers[w])
+            d = np.abs(inst.get_scalers(w).astype(np.float64) - ref.scalers[w])
+            worst = float((d / node_bar[w]).max())
+            assert worst <= 1.0, f"node scaler {w}: {worst:.2f} x the float64 bar"
+            used = max(used, worst)
+    if ref.site is not None:
+        steps = int((sp.ops["scale_write"] >= 0).sum() + (sp.ops["scale_remove"] >= 0).sum())
+        bar = sum(node_bar.values(), np.zeros(pr.C)) + steps * half_ulp(np.abs(ref.site_src) + np.abs(ref.site))
+        d = np.abs(inst.get_scalers(sp.site_dst).astype(np.float64) - ref.site)
+        worst = float((d / np.maximum(bar, 1e-300)).max())
+        assert worst <= 1.0, f"site scaler {sp.site_dst}: {worst:.2f} x the float64 bar"
+        used = max(used, worst)
+    if ref.lnl is not None and lnl is not None:
+        assert status == (abi.EVAL_UNDERFLOW if ref.underflow else abi.EVAL_OK), f"status {status}"
+        if not ref.underflow:
+            cond = pr.uncompressed * 2e-6 * ref.p_un / (1.0 - ref.p_un) if ref.p_un else 0.0
+            bar = lnl_tol(S) * abs(ref.lnl) + cond
+            worst = abs(lnl - ref.lnl) / bar
+            assert worst <= 1.0, f"lnL {lnl!r} vs float64 {ref.lnl!r}: {worst:.2f} x the bar"
+            used = max(used, worst)
+    return used
+
+
+# ---- caller data: seeded buffers and foreign matrices -------------------------------------------------------------
+def _host_layout(pr, x):
+    """[K, C, S] -> the host layout of pr's partials (ragged for variable-state divisions)"""
+    from f64_reference import is_variable_states, padded_to_ragged
+    return padded_to_ragged(pr, x).astype(np.float32) if is_variable_states(pr) else x.astype(np.float32)
+
+
+def seeded_partials(pr, rng):
+    """Interior partials a caller might hold, in pr's host layout: every pattern peaks (0.5 to 1) in a category of its
+    own, the other categories lie 1 to 1e-6 below; about 15 % of the entries are exact zeros and 5 % sit just above
+    FLT_MIN.  Every pattern keeps its peak, so no pattern is zero throughout."""
+    from f64_reference import is_variable_states
+    K, C, S = pr.K, pr.C, pr.S
+    x = rng.uniform(0.0, 1.0, (K, C, S)) ** 2
+    top = rng.integers(0, K, C)
+    x *= np.where(np.arange(K)[:, None] == top[None, :], 1.0, 10.0 ** -rng.uniform(0, 6, (K, C)))[:, :, None]
+    x[rng.random(x.shape) < 0.15] = 0.0
+    tiny = rng.random(x.shape) < 0.05
+    x[tiny] = FLT_MIN * rng.uniform(1.0, 4.0, int(tiny.sum()))
+    n = pr.state_counts if is_variable_states(pr) else np.full(C, S)
+    x[:, np.arange(S)[None, :] >= n[:, None]] = 0.0
+    x[top, np.arange(C), rng.integers(0, 1 << 30, C) % n] = rng.uniform(0.5, 1.0, C)
+    return _host_layout(pr, x)
+
+
+def seeded_scalers(pr, rng, depth):
+    """a scaler buffer: log-peaks down to -depth, some exactly 0"""
+    v = -rng.uniform(0.0, depth, pr.C)
+    v[rng.random(pr.C) < 0.1] = 0.0
+    return v.astype(np.float32)
+
+
+def foreign_rows(n, rng):
+    """[n, n] row-stochastic, non-reversible: a diagonal of 0.3 to 0.9 and Dirichlet rows off it; some rows have
+    exact zeros, some entries of 1e-30 or subnormal, some rows are identity rows.  Row 0 is positive throughout, so that
+    every node keeps a positive entry in state 0 of every category and no pattern's product vanishes."""
+    P = np.zeros((n, n))
+    for i in range(n):
+        d = rng.uniform(0.3, 0.9)
+        off = rng.dirichlet(np.full(n - 1, 0.5)) * (1.0 - d)
+        u = rng.random() if i > 0 else 1.0
+        if u < 0.1:
+            d, off = 1.0, np.zeros(n - 1)                        # identity row
+        elif u < 0.3:
+            off[rng.random(n - 1) < 0.5] = 0.0                   # exact zeros
+        elif u < 0.5:
+            j = rng.integers(0, n - 1, 2)
+            off[j[0]] = 1e-30 * rng.uniform(0.5, 2.0)
+            off[j[1]] = 1e-40 * rng.uniform(0.5, 2.0)            # subnormal in float
+        P[i] = np.insert(off, i, d)
+    return P
+
+
+def foreign_matrix(pr, rng):
+    """a transition-matrix buffer of foreign_rows in pr's host layout: [K, S, S], or a variable-state block with one
+    such matrix per state-count class and category"""
+    from f64_reference import is_variable_states, std_pattern_classes
+    if not is_variable_states(pr):
+        return np.stack([foreign_rows(pr.S, rng) for _ in range(pr.K)]).astype(np.float32)
+    blk = np.zeros(pr.matrix_length, np.float32)
+    for n, ti, _ in std_pattern_classes(pr):
+        for k in range(pr.K):
+            blk[ti + k * n * n: ti + (k + 1) * n * n] = foreign_rows(n, rng).ravel()
+    return blk
+
+
+def seed_chain(insts, pr, ch, rng, depth=30.0):
+    """set_partials / set_scalers, identically on every instance, of chain ch's current interior partials, node scalers
+    and site scaler: the clean operands, removed scalers and site_scaler_src of its next branch update"""
+    st, tr = pr.chains[ch], pr.tree[ch]
+    for p in tr.post:
+        x = seeded_partials(pr, rng)
+        for inst in insts:
+            inst.set_partials(int(st.cl[p]), x)
+        if st.scaled[p]:
+            v = seeded_scalers(pr, rng, depth)
+            for inst in insts:
+                inst.set_scalers(int(st.ns[p]), v)
+    v = seeded_scalers(pr, rng, depth * 5)
+    for inst in insts:
+        inst.set_scalers(int(st.site), v)

@@ -360,3 +360,166 @@ def balanced_tree(n, rng, mean_len=0.1):
 
     build(0, n - 1)
     return _tree(n, left, right, rng, mean_len)
+
+
+# ----------------------------------------------------------------------------- one evaluation over explicit buffers
+FLAG_TIP_SHORTCUTS = 2                        # MB200_FLAG_TIP_SHORTCUTS (include/mb200.h)
+NONE = -1
+
+
+def is_variable_states(pr):
+    return getattr(pr, "state_counts", None) is not None
+
+
+def ragged_to_padded(pr, a):
+    """Std partials: the ragged host layout [K, sum nStates] -> [K, C, S], zeros past each pattern's state count"""
+    off = np.concatenate([[0], np.cumsum(pr.state_counts)])
+    out = np.zeros((pr.K, pr.C, pr.S))
+    for c in range(pr.C):
+        out[:, c, :pr.state_counts[c]] = a[:, off[c]:off[c + 1]]
+    return out
+
+
+def padded_to_ragged(pr, x):
+    return np.concatenate([x[:, c, :pr.state_counts[c]] for c in range(pr.C)], axis=1)
+
+
+def std_mk_block(pr, length, rates):
+    """a variable-state branch's block in float64: expm of each class's Mk rate matrix times clamp(length) r_k, as the
+    engine builds it for a matrix update"""
+    from scipy.linalg import expm
+    blk = np.zeros(pr.matrix_length)
+    v = min(max(float(length), BRLENS_MIN), BRLENS_MAX) * np.asarray(rates, float)
+    for n, ti, _ in std_pattern_classes(pr):
+        for k, vk in enumerate(v):
+            blk[ti + k * n * n: ti + (k + 1) * n * n] = np.maximum(expm(mk_rate_matrix(n) * vk), 0.0).ravel()
+    return blk
+
+
+class Evaluation64:
+    """f64_evaluation's result: every partials buffer the operations wrote (host layout: [K, C, S], ragged for Std),
+    every node scaler they wrote, the site scaler (None without site_dst) and the one it started from, lnL and whether a pattern underflowed (None
+    without a root), and per destination the operations of the call in its subtree, itself included (below) and the
+    largest product before rescaling, per pattern (peak; 1 where the node is not rescaled)"""
+
+    def __init__(self):
+        self.partials, self.scalers, self.below, self.peak = {}, {}, {}, {}
+        self.site = self.site_src = self.lnl = self.underflow = None
+        self.p_un = 0.0
+
+
+def f64_evaluation(pr, sp, partials=None, matrices=None, scalers=None, weights=None, Q=None):
+    """Float64 restatement of one mb200_evaluation over the exact operation list of sp -> Evaluation64.
+
+    The inputs are the buffers the operations read, as the caller holds them: tips from pr.masks; interior partials
+    (partials: buffer -> host layout), P(t) (matrices: matrix -> [K, S, S] or a Std block) and node and site scalers
+    (scalers: buffer -> [C]).  sp's matrix updates are rebuilt here in float64 from the problem's eigensystem, or with Q
+    (per-category rate matrices) by the matrix exponential (transition_matrices; Std: the Mk model), with sp's rates and
+    frequencies, and replace the given ones.  Operations run in order: each child term is
+    P x (a tip's state set as 0/1; with MB200_FLAG_TIP_SHORTCUTS a missing observation on a tip without partial
+    ambiguity is exactly 1), the children multiply, scale_remove leaves the site scaler first, then with scale_write
+    the node is divided by its largest entry per pattern, whose log is the node scaler and joins the site scaler.  A
+    node without scale_write -- the interior root -- is not rescaled.  The site scaler starts from site_scaler_src
+    (zeros without).  The root follows f64_root: ROOT_QUIRK or ROOT_GEN by sp's flags with p_invar, Std's coding-bias
+    correction, weights row `weights` (default the problem's)."""
+    std = is_variable_states(pr)
+    K, C, S = pr.K, pr.C, pr.S
+    weights = np.asarray(pr.weights if weights is None else weights, float)
+    rates, freqs = np.asarray(sp.rates, float), np.asarray(sp.freqs, float)
+    mats = {int(m): np.asarray(v, np.float64) for m, v in (matrices or {}).items()}
+    for mu in sp.mats:
+        m, t = int(mu["matrix"]), float(mu["length"])
+        mats[m] = std_mk_block(pr, t, rates) if std else transition_matrices(pr, t, rates, Q, freqs[:S])
+    given = {int(b): (ragged_to_padded(pr, np.asarray(a, np.float64)) if std else np.asarray(a, np.float64))
+             for b, a in (partials or {}).items()}
+    scal = {int(s): np.asarray(v, np.float64) for s, v in (scalers or {}).items()}
+    n_tips = pr.masks.shape[0]
+    full = np.uint64((1 << S) - 1) if S < 64 else np.uint64(0xFFFFFFFFFFFFFFFF)
+    classes = std_pattern_classes(pr) if std else None
+    out = Evaluation64()
+    cl = {}
+
+    def tip(node):
+        if std:
+            n = pr.state_counts.astype(np.uint64)
+            bits = (pr.masks[node][:, None] >> np.arange(S, dtype=np.uint64)[None, :]) & np.uint64(1)
+            return np.where(np.arange(S)[None, :] < n[:, None], bits, 0).astype(np.float64)
+        return tip_partials(pr, node)
+
+    def ambiguous(node):
+        m = pr.masks[node]
+        return bool(((m != full) & ((m & (m - np.uint64(1))) != 0)).any())
+
+    def term(child, matrix):
+        x = cl[child] if child in cl else given[child] if child >= n_tips else np.broadcast_to(tip(child), (K, C, S))
+        P = mats[matrix]
+        if not std:
+            y = np.einsum("kij,kcj->kci", P, x)
+            if child < n_tips and sp.flags & FLAG_TIP_SHORTCUTS and not ambiguous(child):
+                y[:, pr.masks[child] == full, :] = 1.0
+            return y
+        y = np.zeros((K, C, S))
+        for n, ti, idx in classes:
+            Pk = P[ti:ti + K * n * n].reshape(K, n, n)
+            y[:, idx, :n] = np.einsum("kai,kci->kca", Pk, x[:, idx, :n])
+        return y
+
+    site = scal[sp.site_src].copy() if sp.site_src >= 0 else np.zeros(C)
+    out.site_src = site.copy()
+    for op in sp.ops:
+        dest = int(op["dest"])
+        x = term(int(op["child1"]), int(op["matrix1"])) * term(int(op["child2"]), int(op["matrix2"]))
+        if op["child3"] >= 0:
+            x = x * term(int(op["child3"]), int(op["matrix3"]))
+        if op["scale_remove"] >= 0:
+            r = int(op["scale_remove"])
+            site -= out.scalers[r] if r in out.scalers else scal[r]
+        peak = np.ones(C)
+        if op["scale_write"] >= 0:
+            peak = x.max(axis=(0, 2))
+            peak = np.where(peak > 0, peak, 1.0)
+            x = x / peak[None, :, None]
+            with np.errstate(divide="ignore"):
+                out.scalers[int(op["scale_write"])] = np.log(peak)
+            site += np.log(peak)
+        cl[dest] = x
+        out.peak[dest] = peak
+        out.below[dest] = 1 + sum(out.below.get(int(op[f]), 0) for f in ("child1", "child2", "child3") if op[f] >= n_tips)
+    for dest, x in cl.items():
+        out.partials[dest] = padded_to_ragged(pr, x) if std else x
+    if sp.site_dst >= 0:
+        out.site = site
+    if sp.root < 0:
+        return out
+    root = cl[sp.root] if sp.root in cl else given[sp.root]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        if std:
+            like = np.zeros(C)
+            for n, ti, idx in classes:
+                pi = freqs[pr.freq_offsets[idx][:, None] + np.arange(n)[None, :]]
+                like[idx] = np.einsum("kcj,cj->c", root[:, idx, :n], pi) / K
+            d = pr.dummy
+            out.p_un = float((like[:d] * np.exp(site[:d])).sum())
+            out.underflow = bool((like[d:] < LIKE_EPSILON).any())
+            out.lnl = float((site[d:] + np.log(like[d:])) @ weights[d:]) - \
+                pr.uncompressed * np.log(max(1.0 - out.p_un, LIKE_EPSILON))
+            return out
+        like = np.einsum("k,kcs,s->c", np.asarray(sp.cat_weights, float), root, freqs[:S])
+        if not sp.has_p_invar:
+            out.underflow = bool((like < LIKE_EPSILON).any())
+            out.lnl = float((site + np.log(like)) @ weights)
+            return out
+        inv = np.bitwise_and.reduce(pr.masks, axis=0)
+        bits = (inv[:, None] >> np.arange(S, dtype=np.uint64)[None, :]) & np.uint64(1)
+        p = float(np.float32(sp.p_invar)) if S == 4 else float(sp.p_invar)
+        like_i = p * (bits * freqs[None, :S]).sum(1)
+        rule = root_rule_of(sp.flags)
+        terms, _ = root_site_terms(site, like, like_i, rule)
+        if rule == ROOT_QUIRK:        # the quirk tests the likelihood it takes the log of
+            tested = np.where(site < SCALER_SWITCH, np.where(like_i > LIKE_I_MIN, like_i, like),
+                              like + like_i * np.exp(np.minimum(-site, 700.0)))
+        else:
+            tested = like
+        out.underflow = bool((tested < LIKE_EPSILON).any())
+        out.lnl = float(terms @ weights)
+    return out

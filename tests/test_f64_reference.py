@@ -388,3 +388,69 @@ def test_scaler_drift_bar_long_run(oracle_lib, S, K, C, tips, updates):
             d = np.abs(updated - fresh)
             assert d.max() > 0.0, f"chain {ch}"
             assert (d <= bound + ledger.pattern_bound(fresh_sp)).all(), f"chain {ch}: {d.max():.2e}"
+
+
+# ---- one evaluation over explicit buffers (f64_evaluation) against the oracle, at the shapes of the caller entry-point
+# tests: seeded partials and scalers, caller matrices with exact zeros and tiny entries, Std's ragged layout, +I -------
+EVAL_CASES = {
+    # name: (S, K, C, tips, p_invar, flags or None for the problem's)
+    "nuc4-quirk-I": (4, 4, 90, 9, 0.2, abi.FLAG_NUC4_PINVAR_QUIRK),
+    "nuc4-gen-I": (4, 3, 70, 8, 0.2, 0),
+    "gen16": (16, 2, 45, 7, 0.0, None),
+    "aa20-I": (20, 4, 40, 6, 0.1, 0),
+    "codon61": (61, 1, 20, 5, 0.0, None),
+    "std": None,
+}
+
+
+def eval_problem(name):
+    if EVAL_CASES[name] is None:
+        return workloads.make_std_problem(60, 3, 7, 2, seed=31)
+    S, K, C, tips, pinv, flags = EVAL_CASES[name]
+    return workloads.make_problem(S, K, C, tips, 2, seed=600 + S + K, p_invar=pinv, p_ambig=0.05, flags=flags)
+
+
+def check_oracle_call(o, pr, sp, inputs=None):
+    """sp on the oracle against f64_evaluation of the same call over the buffers it read"""
+    from engine_checks import f64_call_check
+    from f64_reference import f64_evaluation
+    ref = f64_evaluation(pr, sp, *(inputs or ({}, {}, {})))
+    (lo,), (so,) = o.evaluate(sp)
+    return f64_call_check(o, pr, sp, ref, False, so if sp.root >= 0 else None, lo if sp.root >= 0 else None)
+
+
+@pytest.mark.parametrize("name", list(EVAL_CASES))
+def test_f64_evaluation_matches_oracle(oracle_lib, name):
+    """Full evaluations (P(t) rebuilt in float64), branch updates over seeded partials, node scalers and site scalers,
+    and a full evaluation over caller matrices with exact zeros, entries of 1e-30 and subnormal ones and identity rows:
+    every buffer the oracle writes, and lnL, within the float64 bars of f64_call_check, for 4-state +I under both
+    root rules, 16, 20 and 61 states and a Std division whose frequency table is longer than its state count"""
+    from engine_checks import f64_inputs, foreign_matrix, seed_chain
+    pr = eval_problem(name)
+    if name == "std":
+        assert len(pr.freqs) > pr.S
+    rng = np.random.default_rng(5)
+    with pr.create(oracle_lib) as o:
+        o.set_arith(1)
+        for ch in range(pr.n_chains):
+            check_oracle_call(o, pr, pr.full_evaluation(ch))
+        seed_chain([o], pr, 0, rng)
+        removed = 0
+        for it in range(4):
+            sp = pr.random_branch_update(0, rng)
+            assert sp.site_src >= 0
+            removed += int((sp.ops["scale_remove"] >= 0).sum())
+            check_oracle_call(o, pr, sp, f64_inputs(o, sp))
+        assert removed > 0
+        sp = pr.full_evaluation(1)
+        for m in sp.mats["matrix"]:
+            o.set_transition_matrix(int(m), foreign_matrix(pr, rng))
+        sp.mats = sp.mats[:0]
+        check_oracle_call(o, pr, sp, f64_inputs(o, sp))
+        # the root on its own, with the other rule (4 states: the quirk on and off)
+        sp = pr.full_evaluation(0)
+        o.evaluate(sp)
+        root = abi.EvalSpec(site_src=sp.site_dst, root=sp.root, flags=sp.flags ^ abi.FLAG_NUC4_PINVAR_QUIRK,
+                            p_invar=sp.p_invar, has_p_invar=sp.has_p_invar, rates=sp.rates, cat_weights=sp.cat_weights,
+                            freqs=sp.freqs)
+        check_oracle_call(o, pr, root, f64_inputs(o, root))
