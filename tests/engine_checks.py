@@ -240,6 +240,16 @@ def via_replay(e, specs):
     return out
 
 
+def via_replay_begin(e, specs):
+    """pack, then replay_begin / _end: results through the batch's mapped host buffer, on the resident kernel when the
+    engine admits the batch there"""
+    b = e.pack(specs)
+    e.replay_begin(b)
+    out = e.replay_end()
+    e.free_batch(b)
+    return out
+
+
 def resident_generations(e, gens, before=None):
     """generations through replay_begin / _end, all packed first (packing retires a resident kernel); before(g, e),
     if given, runs just before generation g's replay_begin -> [(lnL, status)] per generation"""
@@ -302,6 +312,29 @@ def generation_sequence(pr, gens, seed):
             for ch, sp in enumerate(specs):
                 sp.mats = mats[ch]
                 pr.reject(ch, sp, old[ch])
+
+
+def proposal_cycle(pr, inst, cycle, seed, p_full=0.15, p_accept=0.3):
+    """bench.Job's proposal cycle for one division: every chain's full evaluation on inst now, then cycle - 1 steps of
+    one proposal per chain (a whole-tree evaluation with probability p_full, else a branch update), each rejected with
+    probability 1 - p_accept once its evaluation is built, and a closing step that lands every chain on the state after
+    the full evaluations, so that the cycle can be replayed from its start.  -> [cycle][n_chains] evaluations"""
+    lnl, st = inst.evaluate([pr.full_evaluation(ch) for ch in range(pr.n_chains)])
+    assert not st.any() and np.isfinite(lnl).all()
+    snap = workloads.snapshot(pr)
+    rng = np.random.default_rng(seed)
+    steps = []
+    for _ in range(cycle - 1):
+        specs = []
+        for ch in range(pr.n_chains):
+            old = pr.tree[ch].length.copy()
+            sp = pr.full_evaluation(ch) if rng.random() < p_full else pr.random_branch_update(ch, rng)
+            if rng.random() >= p_accept:
+                pr.reject(ch, sp, old)
+            specs.append(sp)
+        steps.append(specs)
+    steps.append([workloads.reset_evaluation(pr, ch, snap) for ch in range(pr.n_chains)])
+    return steps
 
 
 def assert_resident_equals_launches(engine_lib, oracle_lib, pr, gens, rtol, tol, drift=False):
