@@ -95,6 +95,12 @@ def root_site_terms(lnscale, like, like_i, rule, scalers=None):
     return site, branch
 
 
+def rooted(pr):
+    """a rooted problem (tests/tree_moves.py): the root tip is a dummy no operation reads, the interior root has two
+    children and no branch of its own"""
+    return getattr(pr, "rooted", False)
+
+
 def f64_lnl(pr, ch, tree=None, **kw):
     """-> (per-pattern log likelihoods [C], lnL) of chain `ch` on its current tree: f64_root's"""
     r = f64_root(pr, ch, tree, **kw)
@@ -105,7 +111,8 @@ def f64_root(pr, ch, tree=None, *, Q=None, freqs=None, rates=None, cat_weights=N
              flags=None, rule=None, scalers=None, pmat_cache=None):
     """Float64 pruning of chain `ch` on its current tree -> RootTerms.
 
-    Without overrides the model is the problem's: its eigensystem, frequencies, rates / (1 - p_invar) and
+    On a rooted problem the interior root multiplies its two children only.  Without overrides the model is the
+    problem's: its eigensystem, frequencies, rates / (1 - p_invar) and
     equal category weights (1 - p_invar) / K.  Overrides describe one evaluation's own model: Q (per-category
     rate matrices, see transition_matrices), freqs, rates and cat_weights exactly as the evaluation sends
     them, p_invar (0: none) and the pattern weights of its weights row.  With p_invar the root follows `rule`
@@ -134,9 +141,10 @@ def f64_root(pr, ch, tree=None, *, Q=None, freqs=None, rates=None, cat_weights=N
 
     for p in tr.post:
         x = child(int(tr.left[p])) * child(int(tr.right[p]))
-        if tr.anc[p] == tr.root:                       # the interior root also takes the root tip
-            rt = tip_partials(pr, tr.root)[None]
-            x = x * np.einsum("kij,kcj->kci", pmat(p), np.broadcast_to(rt, x.shape))
+        if tr.anc[p] == tr.root:                       # the interior root also takes the root tip (unrooted)
+            if not rooted(pr):
+                rt = tip_partials(pr, tr.root)[None]
+                x = x * np.einsum("kij,kcj->kci", pmat(p), np.broadcast_to(rt, x.shape))
             # ...and is not rescaled, as in MrBayes: the site scaler holds the other nodes' scalers only, which
             # matters where a root rule adds it to a likelihood it did not scale (ROOT_QUIRK)
             cl[p] = x
@@ -257,7 +265,7 @@ def f64_std_lnl(pr, ch, tree=None, *, rates=None, matrices=None, weights=None):
     Pattern c has n = state_counts[c] states.  P(t) of category k is expm(Q_n v) with v = clamp(length, BRLENS_MIN,
     BRLENS_MAX) * r_k, or, for a branch in `matrices` (node -> the branch's block of matrix_length floats in the host
     layout), the block's [n][n] matrix at matrix_offsets[c] + k n^2, read as row a (parent state), column i (child
-    state).  Pruning with the interior root's three neighbours and per-pattern rescaling by the max over categories
+    state).  Pruning with the interior root's three neighbours (two on a rooted problem) and per-pattern rescaling by the max over categories
     and states.  At the root L_c = 1/K sum_k sum_j pi_j cl[k][c][j], pi = freqs[freq_offsets[c]:] (category weights
     are not used), and lnL = sum_{c >= dummy} w_c log L_c - U log(max(1 - sum_{c < dummy} L_c, LIKE_EPSILON)).
     -> StdLnl"""
@@ -290,7 +298,7 @@ def f64_std_lnl(pr, ch, tree=None, *, rates=None, matrices=None, weights=None):
         l, r = int(tr.left[p]), int(tr.right[p])
         for j, (n, ti, idx) in enumerate(classes):
             x = child(l, j, n, ti, idx) * child(r, j, n, ti, idx)
-            if tr.anc[p] == tr.root:                     # the interior root also takes the root tip
+            if tr.anc[p] == tr.root and not rooted(pr):  # the interior root also takes the root tip (unrooted)
                 x = x * np.einsum("kai,kci->kca", pmat(p, n, ti), np.broadcast_to(tip(tr.root, idx, n), x.shape))
             m = x.max(axis=(0, 2))
             m = np.where(m > 0, m, 1.0)

@@ -14,16 +14,13 @@ small-tree bars, and lnL against float64 within the small-tree bar plus the drif
 The +I tests put the constant patterns' site scalers past -200, where MrBayes stops exponentiating the scaler, on
 every route with invariable sites, under the quirk flag and without it, and show that each branch of the root rule
 was taken.  The largest differences each test measured are printed and recorded as test properties."""
-import dataclasses
-
 import numpy as np
 import pytest
 
-from engine_checks import (SYN_RTOL, assert_resident_equals_launches, check_with_oracle, edge, generation_sequence,
-                           lnl_tol, num_sms, parity_tol, ppb, resident_generations,
-                           subtree_tol, switch_problem, tree_tol, variant_root, via_evaluate, via_replay, with_root_variant)
-from f64_reference import (ABOVE_SWITCH, INVAR_DOMINATES, INVAR_TINY, INVAR_ZERO, ScalerLedger, balanced_tree,
-                           caterpillar_tree, f64_root, f64_std_lnl)
+from engine_checks import (SYN_RTOL, Checker, StdChecker, assert_resident_equals_launches, edge, generation_sequence,
+                           num_sms, parity_tol, ppb, resident_generations, switch_problem, variant_root, via_evaluate,
+                           via_replay, with_root_variant)
+from f64_reference import ABOVE_SWITCH, INVAR_DOMINATES, INVAR_TINY, INVAR_ZERO, balanced_tree, caterpillar_tree
 from mrbayes_b200 import abi, workloads
 
 pytestmark = pytest.mark.gpu
@@ -37,62 +34,6 @@ def install_trees(pr, mean_len=0.1, kinds=None):
         if kind in builders:
             pr.tree[ch] = builders[kind](pr.n_tips, np.random.default_rng(100 + ch), mean_len)
     return pr
-
-
-def large_tree_tol(pr):
-    """subtree_tol, plus 1e-9 of the pattern's largest entry on every partial, and 2.5e-6 instead of 2e-6 relative off
-    the tensor cores (variable-state partials are ragged and keep tree_tol).  On H100, at 300 to 1000 tips, a few
-    entries differed from the oracle's by 1.0 to 1.1 x parity_tol: 4-state at K = 2, entries of 1e-28 of their
-    pattern's largest; the generic kernel at 16 states, entries of 2.5e-6 and 3.7e-4 of the largest, off by up to
-    7e-10 of it, and one of 2e-2, off by 2.03e-6 relative.  That is the float error of P(t)'s small entries and of
-    the summation order, which hundreds of nodes give many chances to show; it moves neither the node's scaler nor
-    lnL, which stay within their bars."""
-    if hasattr(pr, "state_counts"):
-        return tree_tol(pr)
-    base = subtree_tol(pr)
-    rtol = None if pr.S in (20, 61) else 2.5e-6
-
-    def tol(sp):
-        t = dataclasses.replace(base(sp), partials_of_peak=1e-9)
-        return t if rtol is None else dataclasses.replace(t, partials_rtol=rtol)
-    return tol
-
-
-class Checker:
-    """Checks the evaluations of one run in order: lnL, status and every written buffer against the oracle
-    (check_with_oracle, lnl_tol(S) and tree_tol), the site scalers read back into a ScalerLedger, and lnL against
-    float64 (ref(sp, site scalers) -> RootTerms, default f64_root) within lnl_tol(S) |lnL| plus the ledger's drift.
-    Keeps the largest differences relative to lnL, and the largest float64 difference as a fraction of its bar."""
-
-    def __init__(self, pr, e, o, ref=None, rtol=None, tol=None):
-        self.pr, self.e, self.o = pr, e, o
-        self.ref = ref or (lambda sp, sc: f64_root(pr, sp.chain, scalers=sc))
-        self.rtol = lnl_tol(pr.S) if rtol is None else rtol
-        self.tol = tol or large_tree_tol(pr)
-        self.ledger = ScalerLedger()
-        self.worst = {"oracle_rel": 0.0, "partials_rel": 0.0, "f64_rel": 0.0, "f64_of_bar": 0.0}
-        self.branches = set()
-
-    def __call__(self, specs, lnl, st):
-        r, partials_rel, _ = check_with_oracle(self.e, self.o, specs, lnl, st, self.rtol, self.tol)
-        self.worst["oracle_rel"] = max(self.worst["oracle_rel"], r)
-        self.worst["partials_rel"] = max(self.worst["partials_rel"], partials_rel)
-        for i, sp in enumerate(specs):
-            sc = self.e.get_scalers(sp.site_dst)
-            self.ledger.record(sp, sc)
-            ref = self.ref(sp, sc)
-            if getattr(ref, "branch", None) is not None:
-                self.branches |= set(ref.branch.tolist())
-            bar = self.rtol * abs(ref.lnl) + self.ledger.drift(sp, self.pr.weights)
-            d = abs(lnl[i] - ref.lnl)
-            assert d <= bar, f"chain {sp.chain}: engine {lnl[i]!r}, float64 {ref.lnl!r}, bar {bar:.2e}"
-            self.worst["f64_rel"] = max(self.worst["f64_rel"], d / abs(ref.lnl))
-            self.worst["f64_of_bar"] = max(self.worst["f64_of_bar"], d / bar)
-
-    def report(self, record_property, what):
-        for k, v in self.worst.items():
-            record_property(k, v)
-        print(f"\n{what}: " + ", ".join(f"{k} {v:.2e}" for k, v in self.worst.items()))
 
 
 def run(pr, e, o, route, gens, seed, checker, variant=None, before=None):
@@ -225,25 +166,6 @@ def test_generic_large(engine_lib, oracle_lib, record_property, S):
 
 
 # ---- variable-state (Std) ----------------------------------------------------------------------------------------------
-class StdChecker(Checker):
-    """lnL against f64_std_lnl within its bound (StdLnl.bound) plus the drift over the observed patterns; the oracle
-    bar of test_gpu_std"""
-
-    def __call__(self, specs, lnl, st):
-        check_with_oracle(self.e, self.o, specs, lnl, st, 1e-9, self.tol)
-        w = np.asarray(self.pr.weights, np.float64).copy()
-        w[:self.pr.dummy] = 0.0
-        for i, sp in enumerate(specs):
-            self.ledger.record(sp, self.e.get_scalers(sp.site_dst))
-            ref = f64_std_lnl(self.pr, sp.chain)
-            assert not ref.underflow
-            bar = ref.bound(self.pr) + self.ledger.drift(sp, w)
-            d = abs(lnl[i] - ref.lnl)
-            assert d <= bar, f"chain {sp.chain}: engine {lnl[i]!r}, float64 {ref.lnl!r}, bar {bar:.2e}"
-            self.worst["f64_rel"] = max(self.worst["f64_rel"], d / abs(ref.lnl))
-            self.worst["f64_of_bar"] = max(self.worst["f64_of_bar"], d / bar)
-
-
 def test_std_large(engine_lib, oracle_lib, record_property):
     pr = install_trees(workloads.make_std_problem(150, 2, 400, 3, seed=48, max_states=6, dummy=2))
     with pr.create(engine_lib) as e, pr.create(oracle_lib) as o:
